@@ -1,13 +1,14 @@
 #!/usr/bin/env python
 """Benchmark of the Dino U-Net forward path (BASELINE.json metric: 2D 512x512 patches/sec, dinounet_l forward).
 
-    python bench.py --gpus N --steps K --warmup W            # our arm (hand-written sm_100a kernels, C-ABI)
+    python bench.py --gpus N --steps K --warmup W            # our arm (hand-written sm_90a kernels, C-ABI)
     python bench.py --impl reference --gpus N --steps K ...  # the reference's own CPU forward (oracle port) on host cores
 
 One "step" = one forward over one batch of synthetic 3x512x512 patches (per-GPU batch fixed -> weak scaling).  For N>1
 the driver launches one rank per GPU with torch.distributed.run; each rank runs its own batch shard (no data-path
 collective inside the forward) and the step ends with ONE NCCL all-gather of the logits (SURVEY.md section 8e).
-Rank 0 prints exactly one JSON line.
+Rank 0 prints exactly one JSON line.  --dump-outputs DIR writes what the last timed step computed as DIR/<name>.npy
+(inputs and weights are seeded, so two builds can be compared output for output).
 """
 import argparse
 import json
@@ -16,6 +17,8 @@ import subprocess
 import sys
 import threading
 import time
+
+import numpy as np
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
@@ -37,26 +40,44 @@ def parse():
     ap.add_argument("--query-dtype", default="fp32", choices=["16", "fp32"],
                     help="adapter query stream storage: fp32 = the reference's dtype (default), 16 = opt-in reduced storage")
     ap.add_argument("--train-gemm", default="tf32", choices=["tf32", "fp32"],
-                    help="--mode train: matrix products of the trainable part on tcgen05 kind::tf32 (default) or the fp32 SIMT tier")
+                    help="--mode train: matrix products of the trainable part on the TF32 tensor cores (default) or the fp32 SIMT tier")
     ap.add_argument("--no-graph", action="store_true")
-    ap.add_argument("--gemm-pair", default="on", choices=["on", "off"], help="CTA-pair (cta_group::2) GEMM tiles (A/B switch)")
     ap.add_argument("--pdl", default="off", choices=["on", "off"], help="programmatic dependent launch across the plan (A/B switch; measured slower, default off)")
     ap.add_argument("--cpu-sample", type=int, default=8, help="patches in the bounded CPU-baseline sample (0 = skip)")
     ap.add_argument("--eager-steps", type=int, default=10, help="timed steps of the torch-eager CUDA arm at N=1 (0 = skip)")
     ap.add_argument("--ops-out", default="", help="write the per-kernel timing breakdown (JSON) here")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32, <= 64 MB in all); with "
+                         "--gpus N > 1 the all-gathered logits of the whole global batch")
+    a = ap.parse_args()
+    if a.steps < 1:
+        ap.error("--steps must be >= 1")
+    return a
+
+
+DUMP_MAX_ELEMS = 12 * 2 ** 20   # 48 MB of float32 per array; larger outputs are sampled at fixed, seeded positions
+
+
+def dump_outputs(out_dir, arrays):
+    """Host copies of the last timed step's outputs -> out_dir/<name>.npy (float32).  An output with more than DUMP_MAX_ELEMS
+    elements is stored as the values at DUMP_MAX_ELEMS sorted flat positions drawn with a fixed seed (same positions in every
+    run of the same shape)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        a = np.ascontiguousarray(t.detach().float().cpu().numpy().reshape(-1) if hasattr(t, "detach") else np.asarray(t, np.float32).reshape(-1))
+        if a.size > DUMP_MAX_ELEMS:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, DUMP_MAX_ELEMS, replace=False))
+            a = a[idx]
+        np.save(os.path.join(out_dir, f"{name}.npy"), a.astype(np.float32))
 
 
 def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return {"hbm_gbs": d["hbm_gbs"], "tflops": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "src": "measured"}
-    return {"hbm_gbs": 6650.0, "tflops": 1400.0, "src": "fallback"}
+    """Denominators of the roofline fractions: NVIDIA's H100 SXM data sheet (HBM3 bandwidth, dense BF16), not measured."""
+    return {"hbm_gbs": 3350.0, "tflops": 989.0, "src": "H100 SXM data sheet (700 W)"}
 
 
 class ClockSampler:
-    """nvidia-smi clock / throttle-reason sampling (B200_PROFILING.md clocks line).  Started before the warm-up (the tool
+    """nvidia-smi clock / throttle-reason sampling.  Started before the warm-up (the tool
     needs ~1 s to emit its first line); `summary(t0, t1)` keeps only the samples that arrived inside the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -195,8 +216,10 @@ def run_reference(a):
         O.forward(sd, a.model, O.make_input(1, a.size, 0))
     t0 = time.perf_counter()
     for i in range(n):
-        O.forward(sd, a.model, O.make_input(1, a.size, i + 1))   # one step = a bounded sample: 1 patch of the workload
+        y = O.forward(sd, a.model, O.make_input(1, a.size, i + 1))   # one step = a bounded sample: 1 patch of the workload
     dt = time.perf_counter() - t0
+    if a.dump_outputs:
+        dump_outputs(a.dump_outputs, {"logits": y})
     v = n / dt
     print(json.dumps({
         "impl": "reference", "metric": "2D patches/sec (512x512) forward", "value": v, "unit": "patches/s",
@@ -231,9 +254,9 @@ def eager_cuda_patches_per_s(model, B, S, steps, warmup, dev):
 
 
 def run_train(a):
-    """BASELINE.json configs[2]: `dinounet_b random-init, batch 64x512x512x3 synthetic, 1xB200 fwd+bwd (Dice+CE loss)`.
+    """Training step: dinounet_b random-init, synthetic 512x512x3 batches, fwd+bwd (Dice+CE loss).
     One step = nnUNetTrainer.train_step: frozen ViT on the 16-bit tensor-core engine, trainable part forward + backward on the
-    kernels of train_path.py (matrix products: tcgen05 kind::tf32 by default, --train-gemm fp32 = the SIMT parity tier), Dice+CE,
+    kernels of train_path.py (matrix products: TF32 tensor cores by default, --train-gemm fp32 = the SIMT parity tier), Dice+CE,
     (N > 1: one NCCL all-reduce of the gradients), clip + SGD-nesterov."""
     import torch
     import torch.distributed as dist
@@ -279,6 +302,8 @@ def run_train(a):
         if world > 1:
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
         ms = ms.item()
+    if rank == 0 and a.dump_outputs:
+        dump_outputs(a.dump_outputs, {"loss": loss.reshape(1)})
     if rank == 0:
         v = config.VARIANTS[a.model]
         fwd = O.algorithmic_flops_per_patch(a.model, S)
@@ -292,25 +317,25 @@ def run_train(a):
         print(json.dumps({
             "metric": "2D patches/sec (512x512) fwd+bwd (Dice+CE) + SGD step", "value": value, "unit": "patches/s", "n_gpus": world,
             "steps": K, "warmup": W, "ms_per_step": ms / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-            "dtype": ("bf16/fp16 frozen ViT (tcgen05) + trainable part: tf32 tensor-core matrix products (tcgen05 kind::tf32, fp32 "
+            "dtype": ("bf16/fp16 frozen ViT (wgmma) + trainable part: tf32 tensor-core matrix products (wgmma, fp32 "
                       "accumulate), fp32 everything else" if tf32 else
-                      "bf16/fp16 frozen ViT (tcgen05) + fp32 trainable part (SIMT forward/backward kernels)"), "data": "synthetic",
+                      "bf16/fp16 frozen ViT (wgmma) + fp32 trainable part (SIMT forward/backward kernels)"), "data": "synthetic",
             "impl": "b200", "mode": "train",
             "config": {"workload": f"{a.model} train step, {S}x{S}x3, per-GPU batch {B}, Dice+CE, SGD-nesterov + clip 12",
-                       "global_batch": B * world, "l2": "two resident batches alternated; the per-step working set is >> 126 MB L2",
+                       "global_batch": B * world, "l2": "two resident batches alternated; the per-step working set is >> 50 MB L2",
                        "train_gemm": a.train_gemm,
                        "parallelism": f"dp{world} + 1 NCCL all-reduce of the gradients" if world > 1 else "single GPU"},
             "gpu_launches": K * launches_per_step, "kernels_per_step": launches_per_step, "loss": float(loss),
             "clocks": clk.summary(t0, t1),
             "roofline": ({"bound": "tensor", "achieved": value / world * flops / 1e12, "peak": pk["tflops"] / 2, "unit": "TFLOP/s",
                           "frac": value / world * flops / 1e12 / (pk["tflops"] / 2), "algorithmic_gflop_per_patch": flops / 1e9,
-                          "peak_source": "half of the measured sustained bf16 peak (TF32 dense = 0.5 x bf16 on B200; no measured TF32 entry)",
+                          "peak_source": "TF32 dense = 0.5 x the data-sheet bf16 peak",
                           "note": "whole step (frozen ViT + trainable forward/backward + loss + SGD) over the algorithmic FLOPs; the "
                                   "tf32 GEMM's operands go through registers (gathers no tensor map expresses), so it is bound by "
                                   "L2->SM operand traffic and LSU issue, not by the tensor pipe"} if tf32 else
                          {"bound": "fp32-simt", "achieved": value / world * flops / 1e12, "unit": "TFLOP/s",
                           "algorithmic_gflop_per_patch": flops / 1e9,
-                          "note": "fp32 FMA peak of a B200 is ~72 TF/s (148 SMs x 128 lanes x 2 x 1.9 GHz); --train-gemm fp32 runs the "
+                          "note": "fp32 FMA peak of an H100 SXM is 67 TF/s (data sheet); --train-gemm fp32 runs the "
                                   "trainable part on plain fp32 SIMT kernels (the gradient-parity tier)"}),
             "peak_mem_gb": torch.cuda.max_memory_allocated() / 2 ** 30}))
     if world > 1:
@@ -318,7 +343,7 @@ def run_train(a):
 
 
 def run_reference_cuda_train(a):
-    """The reference's training step as torch eager + autograd on the B200 (library kernels, the reference's autocast regime,
+    """The reference's training step as torch eager + autograd on the GPU (library kernels, the reference's autocast regime,
     its differentiable pure-PyTorch deformable-attention core instead of the CUDA extension): forward, Dice+CE, backward, clip,
     SGD-nesterov.  Informational arm beside `--mode train`."""
     import torch
@@ -358,6 +383,8 @@ def run_reference_cuda_train(a):
     e1.record()
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / a.steps
+    if a.dump_outputs:
+        dump_outputs(a.dump_outputs, {"loss": loss.reshape(1)})
     print(json.dumps({"impl": "reference-cuda", "mode": "train", "metric": "2D patches/sec (512x512) fwd+bwd (Dice+CE) + SGD step",
                       "value": B / ms * 1e3, "unit": "patches/s", "n_gpus": 1, "steps": a.steps, "warmup": a.warmup, "ms_per_step": ms,
                       "higher_is_better": True, "dtype": "fp16/bf16 autocast (torch eager + autograd, library kernels)", "data": "synthetic",
@@ -366,7 +393,7 @@ def run_reference_cuda_train(a):
 
 
 def run_reference_cuda(a):
-    """SURVEY.md section 8(d): the same oracle port run by PyTorch eager on the B200 in the reference's GPU precision
+    """SURVEY.md section 8(d): the same oracle port run by PyTorch eager on the GPU in the reference's GPU precision
     regime (outer fp16 autocast, inner bf16 ViT, fp32 MSDA) — what a user gets from the reference code on this GPU
     (cuBLAS/cuDNN/SDPA library kernels).  Informational third arm; not part of the driver contract."""
     import torch
@@ -381,10 +408,12 @@ def run_reference_cuda(a):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for _ in range(a.steps):
-            O.forward(sd, a.model, x, autocast_like_reference=True)
+            y = O.forward(sd, a.model, x, autocast_like_reference=True)
         e1.record()
         torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / a.steps
+    if a.dump_outputs:
+        dump_outputs(a.dump_outputs, {"logits": y})
     print(json.dumps({
         "impl": "reference-cuda", "metric": "2D patches/sec (512x512) forward", "value": a.batch / ms * 1e3,
         "unit": "patches/s", "n_gpus": 1, "steps": a.steps, "warmup": a.warmup, "ms_per_step": ms,
@@ -414,13 +443,12 @@ def main():
     local = int(os.environ.get("LOCAL_RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device (the B200 path has no CPU fallback)")
+        raise SystemExit("bench.py: no CUDA device (the native path has no CPU fallback)")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
         os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
         dist.init_process_group("nccl", device_id=dev)
-    lib.load().b2u_set_option(3, 1 if a.gemm_pair == "off" else 0)
     lib.load().b2u_set_option(5, 1 if a.pdl == "on" else 0)
 
     B, S, K, W = a.batch, a.size, a.steps, max(3, a.warmup)
@@ -438,7 +466,7 @@ def main():
         eng = net._get_engine(dev)
     plan, bufs = eng.get_plan(B, S)
     n_kernels = len(plan.calls)
-    # three resident input batches (3 x 100 MB at B=32 > 126 MB L2) rotated between steps; the per-step activation
+    # three resident input batches (3 x 100 MB at B=32 > 50 MB L2) rotated between steps; the per-step activation
     # working set (GBs) is itself >> L2, so no step starts with a warm cache.
     xs = [O.make_input(B, S, 100 + rank * 7 + i).to(dev) for i in range(3)]
     use_graph = not a.no_graph
@@ -451,7 +479,7 @@ def main():
     def step(i):
         logits, _ = eng.forward(xs[i % 3], use_graph=use_graph)
         if gat is not None:
-            gat.submit(logits)
+            return gat.submit(logits)          # ticket of this step's all-gather
         return logits
 
     with torch.no_grad(), ClockSampler(local) as clk:
@@ -465,12 +493,14 @@ def main():
         t_region0 = time.perf_counter()
         e0.record()
         for i in range(K):
-            step(i)
+            last = step(i)
         if gat is not None:
             gat.wait_all()
         e1.record()
         torch.cuda.synchronize()
         t_region1 = time.perf_counter()
+        if rank == 0 and a.dump_outputs:   # before any later forward reuses the engine's / the gatherer's output buffer
+            dump_outputs(a.dump_outputs, {"logits": gat.result(last) if gat is not None else last})
         if world > 1:
             dist.barrier()
         torch.cuda.synchronize()
@@ -526,28 +556,19 @@ def main():
                     "extractor." + base if name.startswith("e") and name[1].isdigit() else name.split(".")[0])
                 fam[key] = fam.get(key, 0.0) + s_.elapsed_time(e_)
             breakdown = dict(sorted(fam.items(), key=lambda kv: -kv[1]))
-            # dominant kernel: the tcgen05 GEMM family of the ViT (qkv, proj, fc1, fc2) -> tensor-core roofline
+            # dominant kernel: the wgmma GEMM family of the ViT (qkv, proj, fc1, fc2) -> tensor-core roofline
             v = config.VARIANTS[a.model]
             T = B * ((S // 16) ** 2 + config.N_PREFIX)
             flops = v.depth * 2 * T * v.embed_dim * (3 * v.embed_dim + v.embed_dim + 2 * v.ffn_hidden)
             t_gemm = sum(fam.get(k, 0) for k in ("vit.qkv", "vit.proj", "vit.fc1", "vit.fc2"))
             pk = peaks()
-            traffic, traffic_src = None, None
-            tpath = os.path.join(ROOT, "profiles", "r02_traffic.json")
-            tj = None
-            if os.path.exists(tpath) and (a.model, B, S, a.vit_dtype) == ("dinounet_l", 32, 512, "bf16"):
-                # dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed ncu pass over one step of exactly
-                # this workload (tools/one_step.py + tools/ncu_table.py), averaged over the four ViT GEMM shapes
-                tj = json.load(open(tpath))
-                traffic = tj["vit_gemm_family_avg_per_launch"]
-                traffic_src = "profiles/r02_traffic.json (ncu per-launch dram bytes, qkv/proj/fc1/fc2 of one step)"
             ach = flops / (t_gemm * 1e-3) / 1e12
-            roof = {"bound": "tensor", "kernel": "gemm_tc2_kernel<256,EPI,ACT,%s> = persistent tcgen05 GEMM (ViT qkv/proj/fc1/fc2, %d launches/step)" % (a.vit_dtype, 4 * v.depth),
-                    "achieved": ach, "peak": pk["tflops"], "unit": "TFLOP/s", "frac": ach / pk["tflops"], "traffic": traffic, "traffic_source": traffic_src,
+            roof = {"bound": "tensor", "kernel": "gemm_tc2_kernel<128,EPI,ACT,%s> = persistent wgmma GEMM (ViT qkv/proj/fc1/fc2, %d launches/step)" % (a.vit_dtype, 4 * v.depth),
+                    "achieved": ach, "peak": pk["tflops"], "unit": "TFLOP/s", "frac": ach / pk["tflops"],
                     "algorithmic_bytes_per_launch": (T * v.embed_dim * 2 * 2 + T * v.ffn_hidden * 2 * 2 + T * 3 * v.embed_dim * 2 + 2 * T * v.embed_dim * 8
                                                      + 2 * (4 * v.embed_dim * v.embed_dim + 2 * v.embed_dim * v.ffn_hidden)) / 4,
-                    "peak_source": pk["src"] + " (bf16 sustained)", "share_of_step": t_gemm / sum(fam.values())}
-            # top HBM-bound kernel: the 512^2 decoder conv (2f -> f channels, implicit GEMM, halo mode): reads the concat
+                    "peak_source": pk["src"], "share_of_step": t_gemm / sum(fam.values())}
+            # top HBM-bound kernel: the 512^2 decoder conv (2f -> f channels, implicit GEMM): reads the concat
             # buffer once, writes the conv output once (+ the per-(n,c) statistics); SURVEY.md section 8(d): bytes = (Cin+Cout)*2 B/px
             per_op = {n: s_.elapsed_time(e_) for n, s_, e_ in evs}
             f0 = eng.features[0]
@@ -555,15 +576,16 @@ def main():
             t_conv = per_op.get("d2.conv0")
             if t_conv:
                 ach_h = hb / (t_conv * 1e-3) / 1e9
-                roof_hbm = {"bound": "hbm", "kernel": "gemm_tc2_kernel<32,...> conv3x3 halo mode (decoder stage 2 conv 0, %d->%d ch @ %dx%d)" % (2 * f0, f0, S, S),
+                roof_hbm = {"bound": "hbm", "kernel": "gemm_tc2_kernel<32,...> conv3x3 (decoder stage 2 conv 0, %d->%d ch @ %dx%d)" % (2 * f0, f0, S, S),
                             "achieved": ach_h, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": ach_h / pk["hbm_gbs"],
                             "algorithmic_bytes_per_launch": hb, "us": t_conv * 1e3,
-                            "traffic": (tj or {}).get("per_launch_dram_bytes", {}).get("d2.conv0"), "peak_source": pk["src"]}
+                            "peak_source": pk["src"]}
             if a.ops_out:
                 os.makedirs(os.path.dirname(a.ops_out) or ".", exist_ok=True)
                 json.dump({"per_family_ms": breakdown, "per_op_ms": [(n, s_.elapsed_time(e_)) for n, s_, e_ in evs]},
                           open(a.ops_out, "w"), indent=1)
 
+    peak_mem_gb = torch.cuda.max_memory_allocated(dev) / 2 ** 30   # this path only: before the torch-eager comparison arm
     if rank == 0:
         cpu = None
         if a.cpu_sample > 0 and a.model != "dinounet_7b":   # the 7B CPU forward needs ~30 GB and minutes: not a bounded sample
@@ -573,7 +595,7 @@ def main():
         eager = None
         if world == 1 and a.eager_steps > 0 and a.model != "dinounet_7b":
             # the reference algorithm as PyTorch eager on THIS GPU (library kernels, the reference's autocast regime):
-            # the "reference already on Blackwell libraries" bar of SURVEY.md section 8(d), same box, same batch
+            # the "reference on vendor libraries" bar of SURVEY.md section 8(d), same GPU, same batch
             eng.clear_plans()
             torch.cuda.empty_cache()
             eager = eager_cuda_patches_per_s(a.model, B, S, a.eager_steps, 3, dev)
@@ -585,7 +607,7 @@ def main():
             "data": "synthetic", "impl": "b200",
             "config": {"workload": f"{a.model} forward, {S}x{S}x3, per-GPU batch {B}, random-init weights" + (" (generated on device)" if a.model == "dinounet_7b" else " (seed 0)"),
                        "global_batch": B * world, "parallelism": f"batch-sharded dp{world} + 1 NCCL all-gather of fp16 logits per step (side stream, double-buffered)" if world > 1 else "single GPU",
-                       "l2": "3 resident input batches rotated (3x%.0f MB) and a per-step activation working set >> 126 MB L2" % (B * 3 * S * S * 4 / 1e6),
+                       "l2": "3 resident input batches rotated (3x%.0f MB) and a per-step activation working set >> 50 MB L2" % (B * 3 * S * S * 4 / 1e6),
                        "cuda_graph": use_graph, "programmatic_dependent_launch": a.pdl == "on"},
             "e2e": {"value": e2e, "unit": "patches/s", "h2d_bytes_per_step": B * 3 * S * S * 4,
                     "d2h_bytes_per_step": B * 2 * S * S * 4},
@@ -594,6 +616,7 @@ def main():
             "roofline": roof, "roofline_hbm": roof_hbm, "cpu_baseline": cpu, "eager_cuda": eager,
             "model_tflops": value / world * total_flops / 1e12,
             "breakdown_ms": {k: round(v, 3) for k, v in list(breakdown.items())[:14]},
+            "peak_mem_gb": peak_mem_gb,
         }
         print(json.dumps(out))
     if world > 1:

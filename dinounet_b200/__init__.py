@@ -1,4 +1,4 @@
-"""dinounet_b200 — B200-native (sm_100a) implementation of the Dino U-Net forward segmentation path.
+"""dinounet_b200 — H100-native (sm_90a) implementation of the Dino U-Net forward segmentation path.
 
 Public surface (drop-in for the reference's `dinounet_training.py` model + trainer hook):
     from dinounet_b200 import DinoUNet, DinoUNetTrainer_s/_b/_l/_7b, get_dinov3_trainer

@@ -1,4 +1,4 @@
-"""Loading nnU-Net / Dino U-Net training checkpoints (`checkpoint_final.pth`, `checkpoint_best.pth`) into the B200 model.
+"""Loading nnU-Net / Dino U-Net training checkpoints (`checkpoint_final.pth`, `checkpoint_best.pth`) into the native model.
 
 The reference writes `{'network_weights': state_dict, 'optimizer_state', 'grad_scaler_state', 'logging', '_best_ema',
 'current_epoch', 'init_args', 'trainer_name', 'inference_allowed_mirroring_axes'}` (nnUNetTrainer.py:1083-1104) and reads

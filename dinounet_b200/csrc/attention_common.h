@@ -1,4 +1,4 @@
-// Shared by the tcgen05 attention kernels (attention_tc.cu: host entry points + few-row companion, attention_tc3.cu: kernel).
+// Shared by the attention translation units (attention_tc.cu: host entry points + few-row companion, attention_tc3.cu: kernel).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -12,10 +12,10 @@ struct alignas(64) AttnMaps {
   CUtensorMap q, k, vt;
 };
 struct AttnArgs {
-  int BH, heads, ntok, npairs, nchunks;
+  int BH, heads, ntok, nchunks;
   int q_begin;      // first query row handled by this launch (rows [q_begin, ntok)); keys always span [0, ntok)
-  int pairs_full;   // head_dim 64: items [0, BH*pairs_full) are full tile pairs, the rest single leftover tiles
-  long long items;
+  int qtiles;       // 128-row query tiles per (batch, head)
+  long long items;  // BH * qtiles: one CTA each
   float scale_log2e;
   void* out;
 };
@@ -41,6 +41,6 @@ __device__ __forceinline__ float ex2(float x) {
   return r;
 }
 
-int attention_tc3_dispatch(const AttnMaps& maps, const AttnArgs& a, int head_dim, int dtype, int variant, cudaStream_t stream);
+int attention_tc3_dispatch(const AttnMaps& maps, const AttnArgs& a, int head_dim, int dtype, cudaStream_t stream);
 
 }  // namespace b2u

@@ -1,7 +1,4 @@
-// Host entry points of the tcgen05 / TMEM flash attention (kernel: attention_tc3.cu) and its few-row companion kernel.
-// Round-2 history: the second-generation kernel that lived here (two TMEM passes over S per chunk, O in registers, one
-// polling MMA issuer: 352 us/layer at the bench shape) was replaced by attention_tc3.cu (263 us); a fourth-generation
-// experiment (64-key chunks, double-buffered S and P) was measured at 383 us and dropped.  profiles/r02_attention_ab.json.
+// Host entry points of the wgmma flash attention (kernel: attention_tc3.cu) and its few-row companion kernel.
 // Replaces F.scaled_dot_product_attention at dinounet/dinov3/layers/attention.py:116.
 #include <type_traits>
 
@@ -199,21 +196,17 @@ static int attention_tc_impl(const void* q, const void* k, const void* vt, void*
   a.ntok = ntok;
   a.q_begin = q_begin;
   a.nchunks = (ntok + 127) / 128;
-  const int groups = head_dim == 64 ? 2 : 1;
-  const int ntiles = (ntok - q_begin + 127) / 128;
-  a.npairs = (ntiles + groups - 1) / groups;
-  a.pairs_full = ntiles / groups;
-  a.items = static_cast<long long>(a.BH) * a.npairs;
+  a.qtiles = (ntok - q_begin + 127) / 128;
+  a.items = static_cast<long long>(a.BH) * a.qtiles;
   a.scale_log2e = scale * 1.4426950408889634f;
   a.out = out;
   int rc;
   const uint64_t BH = static_cast<uint64_t>(a.BH), hd = static_cast<uint64_t>(head_dim);
-  // option 4 = 4 (A/B switch): the single-pass softmax variant of the kernel (64 live scores; measured slower at head_dim 64)
   const uint32_t kc = 128u;
   if ((rc = make_map_3d(&maps.q, q, dtype, hd, ntok, BH, hd, static_cast<uint64_t>(ntok) * hd, 64, 128))) return rc;
   if ((rc = make_map_3d(&maps.k, k, dtype, hd, ntok, BH, hd, static_cast<uint64_t>(ntok) * hd, 64, kc))) return rc;
   if ((rc = make_map_3d(&maps.vt, vt, dtype, npad, hd, BH, npad, static_cast<uint64_t>(npad) * hd, 64, static_cast<uint32_t>(head_dim)))) return rc;
-  return attention_tc3_dispatch(maps, a, head_dim, dtype, get_option(4), stream);
+  return attention_tc3_dispatch(maps, a, head_dim, dtype, stream);
 }
 
 extern "C" int b2u_attention_tc(const void* q, const void* k, const void* vt, void* out, int32_t B, int32_t heads,

@@ -1,533 +1,190 @@
-// tcgen05 / TMEM flash attention for the DINOv3 ViT, third generation (head_dim 64 / 128, non-causal, ntok = 1029 at 512^2).
+// Flash attention on the sm_90a warpgroup MMA for the DINOv3 ViT (head_dim 64 / 128, non-causal, ntok = 1029 at 512^2).
 // Replaces F.scaled_dot_product_attention at dinounet/dinov3/layers/attention.py:116 (math: :106-118).
 //
-// Persistent CTAs (1 per SM).  One work item = (batch*head, pair of 128-row query tiles) [head_dim 128: one tile]:
-//   warp 0        : TMA producer — Q tiles (once per item), K chunk [128 keys x HD] + V^T chunk [HD x 128 keys] ring
-//   warp 1        : MMA issuer: one thread running an event loop over both query-tile groups (non-blocking barrier polls,
-//                   so group B's S never queues behind a wait for group A's P):
-//                                   S_g(j) = Q_g K_j^T  -> TMEM S_g        (M128 N128 K=HD)
-//                                   O_g   += P_g(j) V_j -> TMEM O_g        (M128 N=HD K128, accumulates IN TMEM over j)
-//   softmax warps : 2 warps per (group, TMEM lane quarter), each owning 64 of the 128 score columns of its 32 rows:
-//                   ONE tcgen05.ld pass: S -> registers (the S buffer is released to the issuer right after the load, so
-//                   S(j+1) is produced while this chunk's exponentials run), row max, exp2, 16-bit P into 128B-swizzled
-//                   smem (A operand of the PV MMA).
-// What changed against the second generation (attention_tc.cu in round 1: 388 us/layer, 2 TMEM passes over S per chunk +
-// an O read-modify-write in registers per chunk):
-//   * O lives in TMEM for the whole item; the running maximum is updated LAZILY (only when it grows by more than 2^8,
-//     as flash-attention 4 does), so the common chunk does no O traffic at all; the rare rescale is a tcgen05.ld /
-//     tcgen05.st round trip of the warp's O slice between two PV MMAs.
-//   * the last key chunk is as wide as it needs to be (ntok = 1029 -> 16 keys instead of 128: S MMA N = 16, one K = 16
-//     PV MMA, softmax over one 32-column group), and softmax warps whose 32 query rows are all beyond ntok (3 of the 4
-//     quarters of the 5-row ninth tile) only keep the barrier protocol alive.
-//   * items are ordered long-first: all full tile pairs, then the single-tile leftovers, so the persistent round-robin
-//     ends on the short items.
-// Every MMA operand is K-major SW128; V is consumed as V^T [B,H,HD,npad] (written transposed by the QKV epilogue).
-// TMEM columns per group: S [0,128) | O [128, 128+HD) | P [128+HD, 128+HD+64) (16-bit probabilities, A operand of the PV MMA).
-#include <type_traits>
-
+// One CTA per (batch*head, 128-row query tile), 288 threads:
+//   warp 8     : TMA producer - the Q tile once, then a 2-stage ring of {K chunk [128 keys x HD], V^T chunk [HD x 128 keys]}
+//   warps 0-7  : two consumer warpgroups, 64 query rows each.  Per key chunk j:
+//                  S = Q K_j^T        wgmma m64n128k16, both operands from shared memory, S in registers
+//                  online softmax     row max over the 4 lanes that share a row, P = exp2(S * scale*log2(e) - m), O *= corr
+//                  O += P V_j         wgmma m64nHDk16 with P as the REGISTER A operand: the accumulator fragment of S for
+//                                     16 key columns is exactly the A fragment of one K = 16 step, so P never touches smem
+//                and release the stage.  Scores of keys >= ntok are -inf (P = 0 exactly), so every chunk runs the same 8 PV
+//                steps: the V^T padding is zero (callers zero it, TMA zero-fills past npad), and no wgmma sits in a branch.
+// Occupancy: one CTA per SM.  The S, O and P fragments take 168 registers x 288 threads; two CTAs would need <= 113
+// registers per thread, and at that cap (ptxas: 96) the fragments spill to local memory (0.8 KB at head_dim 64, 4 KB at
+// 128).  The two consumer warpgroups run their chunks independently, so one's softmax can overlap the other's MMAs.
+// Every shared-memory operand is K-major SW128; V is consumed as V^T [B,H,HD,npad] (written transposed by the QKV epilogue).
 #include "common.cuh"
 #include "../../include/dinounet_b200.h"
 #include "host_util.h"
 #include "gemm_common.h"
 #include "attention_common.h"
+#include "wgmma.cuh"
 
 namespace b2u {
 
-template <int HD> struct At3Cfg {
-  static constexpr int kGroups = HD == 64 ? 2 : 1;
-  static constexpr int kSplit = 2;
-  static constexpr int kStages = HD == 64 ? 3 : 2;
+template <int HD> struct AttCfg {
+  static constexpr int kStages = 2;
   static constexpr int kKB = HD / 64;                       // 64-wide K blocks of the head dim
-  static constexpr int kQBytes = 128 * HD * 2;
-  static constexpr int kPBytes = 2 * 128 * 128;             // two key blocks of [128 rows x 64 keys]
-  static constexpr int kKBytes = 128 * HD * 2;
+  static constexpr int kQBytes = 128 * HD * 2;              // kKB blocks of [128 rows x 64 dims]
+  static constexpr int kKBytes = 128 * HD * 2;              // kKB blocks of [128 keys x 64 dims]
   static constexpr int kVBytes = 2 * HD * 128;              // two key blocks of [HD rows x 64 keys]
-  static constexpr int kCtrlWarps = 4;                      // TMA producer, MMA issuer A, MMA issuer B, (idle)
-  // 20 warps compile to 96 registers per thread (registers are allocated per 4-warp granule: 65536 / 640)
-  static constexpr int kThreads = kCtrlWarps * 32 + kGroups * 128 * kSplit;
-  static constexpr int kXchgBytes = 2 * 128 * 4 * 4;        // [2 groups][128 rows][4] fp32 exchange slots
-  static constexpr int kGroupCols = 128 + HD + 64;          // S | O | P (128 keys x 16 bit = 64 columns)
-  static constexpr int kSmem = kGroups * (kQBytes + kPBytes) + kStages * (kKBytes + kVBytes) + 1024 + 256 + kXchgBytes;
+  static constexpr int kConsumerWarps = 8;
+  static constexpr int kThreads = 32 * kConsumerWarps + 32;
+  static constexpr int kSmem = kQBytes + kStages * (kKBytes + kVBytes) + 1024 + 256;
 };
 
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]),
-      "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]),
-      "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st4(uint32_t taddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};" ::"r"(taddr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// item -> (bh, pair, number of query tiles in it).  Full pairs first, leftover single tiles last.
-struct ItemDec {
-  int bh, pair, nq;
-};
-template <int NG>
-__device__ __forceinline__ ItemDec decode_item(long long item, const AttnArgs& a) {
-  ItemDec d;
-  if (NG == 1) {
-    d.bh = static_cast<int>(item / a.npairs);
-    d.pair = static_cast<int>(item - static_cast<long long>(d.bh) * a.npairs);
-    d.nq = 1;
-    return d;
-  }
-  const long long nfull = static_cast<long long>(a.BH) * a.pairs_full;
-  if (item < nfull) {
-    d.bh = static_cast<int>(item / a.pairs_full);
-    d.pair = static_cast<int>(item - static_cast<long long>(d.bh) * a.pairs_full);
-    d.nq = 2;
-  } else {
-    d.bh = static_cast<int>(item - nfull);
-    d.pair = a.pairs_full;
-    d.nq = 1;
-  }
-  return d;
-}
-
-// Row maximum over one 32-column group of raw scores; only the last key chunk (kTail) has columns >= lim to skip.
-// Four independent accumulators: a single running maximum is a 32-deep dependent FMNMX chain (~4 cycles each).
-template <bool kTail>
-__device__ __forceinline__ float row_max(const uint32_t (&v)[32], int lim, float mx) {
-  float a[4] = {mx, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-  for (int c = 0; c < 32; ++c) {
-    if (kTail) {
-      if (c < lim) a[c & 3] = fmaxf(a[c & 3], __uint_as_float(v[c]));
-    } else {
-      a[c & 3] = fmaxf(a[c & 3], __uint_as_float(v[c]));
-    }
-  }
-  return fmaxf(fmaxf(a[0], a[1]), fmaxf(a[2], a[3]));
-}
-
-// One 32-column group: P = exp2(s*scale - m) -> 16-bit -> swizzled smem (A operand of the PV MMA); returns the fp32 row
-// sum of the un-rounded probabilities (as flash-attention).  gc = index of the group inside the 128-key chunk:
-// K-block gc>>1, 16-byte chunks (gc&1)*4 .. +3 of this row.  Two compiled bodies: only the last key chunk zeroes columns.
-// exp2 on the FMA / ALU pipes (Cody-Waite split + degree-3 minimax polynomial, max rel err 7.5e-5 - far below the 16-bit
-// rounding of P): x = n + f, f in [-0.5, 0.5]; 2^f ~ c0 + f (c1 + f (c2 + f c3)); 2^n by adding n to the exponent field.
-// Used for every POLY-th probability (default: every 3rd) so that the MUFU pipe (16 exp2 / clk / SM: the roofline of
-// head_dim-64 attention) is relieved of a third of its work (flash-attention 4 does the same).
-__device__ __forceinline__ float ex2_poly(float x) {
-  x = fmaxf(x, -125.0f);
-  const float xf = x + 12582912.0f;                 // 1.5 * 2^23: the integer part lands in the low mantissa bits
-  const float f = x - (xf - 12582912.0f);
-  float p = fmaf(0.05517165f, f, 0.24261113f);
-  p = fmaf(p, f, 0.69326097f);
-  p = fmaf(p, f, 0.99992806f);
-  return __int_as_float(__float_as_int(p) + (__float_as_int(xf) << 23));
-}
-
-template <typename TT, bool kTail, int POLY, bool PT>
-__device__ __forceinline__ float exp_store(const uint32_t (&v)[32], int lim, float sl2, float m_new, int gc,
-                                           uint32_t sP_row, int row, uint32_t tP) {
-  float2 rs2[4] = {{0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}};    // independent packed partial sums
-  const float2 sl2v = make_float2(sl2, sl2), mnv = make_float2(-m_new, -m_new);
-  const uint32_t base = sP_row + (gc >> 1) * (128 * 128);
-#pragma unroll
-  for (int c4 = 0; c4 < 4; ++c4) {       // 8 probabilities -> one 16-byte store
-    uint32_t pk[4];
-#pragma unroll
-    for (int c = 0; c < 8; c += 2) {
-      const int cc = c4 * 8 + c;
-      const float2 xx = fma2(make_float2(__uint_as_float(v[cc]), __uint_as_float(v[cc + 1])), sl2v, mnv);
-      float a = (POLY > 0 && (cc % POLY) == POLY - 1) ? ex2_poly(xx.x) : ex2(xx.x);
-      float b = (POLY > 0 && ((cc + 1) % POLY) == POLY - 1) ? ex2_poly(xx.y) : ex2(xx.y);
-      if constexpr (kTail) {
-        if (cc >= lim) a = 0.f;
-        if (cc + 1 >= lim) b = 0.f;
-      }
-      rs2[c >> 1] = add2(rs2[c >> 1], make_float2(a, b));
-      pk[c >> 1] = TT::pack2(a, b);
-    }
-    if constexpr (PT) {
-      tmem_st4(tP + gc * 16 + c4 * 4, pk[0], pk[1], pk[2], pk[3]);   // keys gc*32 + c4*8 .. +7 of this thread's row
-    } else {
-      const int chunk = (gc & 1) * 4 + c4;
-      sts128a(base + ((chunk ^ (row & 7)) << 4), pk[0], pk[1], pk[2], pk[3]);
-    }
-  }
-  const float2 t = add2(add2(rs2[0], rs2[1]), add2(rs2[2], rs2[3]));
-  return t.x + t.y;
-}
-
-struct SmCtx {
-  uint32_t tS, tO, tP, sP_row;
-  int row, part, lane, bar_id;
-  float* xm;
-  float sl2;
-  uint64_t *s_full, *s_free, *p_full, *o_full;
-};
-
-// One key chunk of the online softmax for the 32 query rows x 64 score columns of one warp.
-//   !kTail: one and a half TMEM passes with 32 scores live at a time (64 live scores + state do not fit the 96 registers
-//           a >512-thread CTA compiles to): group 0 -> max, group 1 -> max (kept), exchange with the partner warp,
-//           exp(group 1), re-read group 0, release S, exp(group 0).  Every tcgen05.ld is unconditional: an asm output
-//           array defined under a branch is materialised in local memory by the compiler.
-//    kTail: the last chunk owns ngrp in {0,1,2} groups and lim valid columns: per-group blocks with their own arrays.
-template <typename TT, int HD, bool kTail, bool kOne, int POLY, bool PT>
-__device__ __forceinline__ void softmax_chunk(const SmCtx& cx, int j, int ngrp, int lim, float& m, float& l,
-                                              uint32_t& sfull_cnt, uint32_t& ofull_cnt) {
-  constexpr int OW = HD / 2;
-  mbar_wait(cx.s_full, sfull_cnt & 1);
-  ++sfull_cnt;
-  tc_fence_after();
-  float mx = -INFINITY, rs = 0.f;
-  uint32_t v[32];
-  uint32_t w[32];   // kOne only
-  if constexpr (!kTail && kOne) {
-    // single TMEM pass, 64 scores live (a few registers spill at the 96-register cap of a >512-thread CTA)
-    tmem_ld32(cx.tS, w);
-    tmem_ld32(cx.tS + 32, v);
-    tmem_ld_wait();
-    tc_fence_before();
-    __syncwarp();
-    if (cx.lane == 0) mbar_arrive(cx.s_free);                // S(j) is in registers: S(j+1) may be produced
-    mx = row_max<false>(w, 32, mx);
-    mx = row_max<false>(v, 32, mx);
-  } else if constexpr (!kTail) {
-    tmem_ld32(cx.tS, v);
-    tmem_ld_wait();
-    mx = row_max<false>(v, 32, mx);
-    tmem_ld32(cx.tS + 32, v);
-    tmem_ld_wait();
-    mx = row_max<false>(v, 32, mx);
-  } else {
-#pragma unroll
-    for (int pc = 0; pc < 2; ++pc) {
-      if (pc < ngrp) {
-        uint32_t t[32];
-        tmem_ld32(cx.tS + pc * 32, t);
-        tmem_ld_wait();
-        mx = row_max<true>(t, lim - pc * 32, mx);
-      }
-    }
-  }
-  cx.xm[(j & 1) * 2 + cx.part] = mx;
-  asm volatile("bar.sync %0, 64;" ::"r"(cx.bar_id) : "memory");
-  mx = fmaxf(mx, cx.xm[(j & 1) * 2 + (cx.part ^ 1)]);
-  const float m_cand = fmaxf(m, mx * cx.sl2);                // chunk 0 always has valid keys -> finite
-  const bool need = (m_cand - m) > 8.0f;                     // lazy: keep the old reference while exp2 stays <= 2^8
-  float m_new = m, corr = 1.f;
-  if (need) { m_new = m_cand; corr = ex2(m - m_new); }
-  if (j > 0) {                                               // PV(j-1) retired: P smem is free, O is quiescent
-    mbar_wait(cx.o_full, ofull_cnt & 1);
-    ++ofull_cnt;
-    tc_fence_after();
-  }
-  if constexpr (!kTail) {
-    rs = exp_store<TT, false, POLY, PT>(v, 32, cx.sl2, m_new, cx.part * 2 + 1, cx.sP_row, cx.row, cx.tP);
-    if constexpr (kOne) {
-      rs += exp_store<TT, false, POLY, PT>(w, 32, cx.sl2, m_new, cx.part * 2, cx.sP_row, cx.row, cx.tP);
-    } else {
-      tmem_ld32(cx.tS, v);
-      tmem_ld_wait();
-    }
-  } else {
-#pragma unroll
-    for (int pc = 0; pc < 2; ++pc) {
-      if (pc < ngrp) {
-        uint32_t t[32];
-        tmem_ld32(cx.tS + pc * 32, t);
-        tmem_ld_wait();
-        rs += exp_store<TT, true, POLY, PT>(t, lim - pc * 32, cx.sl2, m_new, cx.part * 2 + pc, cx.sP_row, cx.row, cx.tP);
-      }
-    }
-  }
-  if constexpr (kTail || !kOne) {
-    tc_fence_before();
-    __syncwarp();
-    if (cx.lane == 0) mbar_arrive(cx.s_free);                // all reads of S(j) done: S(j+1) may be produced
-    if constexpr (!kTail) rs += exp_store<TT, false, POLY, PT>(v, 32, cx.sl2, m_new, cx.part * 2, cx.sP_row, cx.row, cx.tP);
-  }
-  // ---- rare: the reference maximum moved -> rescale this warp's slice of O in TMEM (no PV MMA is in flight: PV(j-1) has
-  // retired and PV(j) waits for this warp's p_full arrival)
-  if (j > 0 && __any_sync(0xffffffffu, need)) {
-#pragma unroll
-    for (int h = 0; h < OW / 32; ++h) {
-      uint32_t o[32];
-      tmem_ld32(cx.tO + h * 32, o);
-      tmem_ld_wait();
-#pragma unroll
-      for (int c = 0; c < 32; ++c) o[c] = __float_as_uint(__uint_as_float(o[c]) * corr);
-      tmem_st32(cx.tO + h * 32, o);
-    }
-    tmem_st_wait();
-  }
-  l = l * corr + rs;
-  m = m_new;
-  if constexpr (PT) tmem_st_wait();          // P (and a rescaled O) are in tensor memory before the MMA is told so
-  else fence_proxy_async();                  // make the generic-proxy P writes visible to the MMA (async proxy)
-  tc_fence_before();
-  __syncwarp();
-  if (cx.lane == 0) mbar_arrive(cx.p_full);
-}
-
-template <typename T, int HD, bool kOne, int POLY, bool PT>
-__global__ void __launch_bounds__(At3Cfg<HD>::kThreads, 1) attn_tc3_kernel(const __grid_constant__ AttnMaps maps, const AttnArgs args) {
+template <typename T, int HD>
+__global__ void __launch_bounds__(AttCfg<HD>::kThreads, 1) attn_tc3_kernel(const __grid_constant__ AttnMaps maps, const AttnArgs args) {
   using TT = T16<T>;
-  using CF = At3Cfg<HD>;
-  constexpr int NG = CF::kGroups, NST = CF::kStages, KB = CF::kKB, SPLIT = CF::kSplit;
-  constexpr int kArr = 4 * SPLIT;                    // one arrival per softmax warp of a group
+  using CF = AttCfg<HD>;
+  constexpr int KB = CF::kKB, NST = CF::kStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;                               // [NG][kQBytes]
-  uint8_t* sP = sQ + NG * CF::kQBytes;              // [NG][32 KB]
-  uint8_t* sK = sP + NG * CF::kPBytes;              // [stages][kKBytes]
+  uint8_t* sQ = smem;
+  uint8_t* sK = sQ + CF::kQBytes;                   // [stages][kKBytes]
   uint8_t* sV = sK + NST * CF::kKBytes;             // [stages][kVBytes]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + NST * CF::kVBytes);
-  uint64_t* q_full = bars;                 // [2]
-  uint64_t* q_free = q_full + 2;           // [2]
-  uint64_t* kv_full = q_free + 2;          // [4]
-  uint64_t* kv_empty = kv_full + 4;        // [4]
-  uint64_t* s_full = kv_empty + 4;         // [2]
-  uint64_t* s_free = s_full + 2;           // [2]
-  uint64_t* p_full = s_free + 2;           // [2]
-  uint64_t* o_full = p_full + 2;           // [2]
-  uint64_t* o_free = o_full + 2;           // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_free + 2);
-  float* xchg = reinterpret_cast<float*>(bars + 32);   // 256 B of barriers, then the exchange slots
+  uint64_t* q_full = reinterpret_cast<uint64_t*>(sV + NST * CF::kVBytes);
+  uint64_t* kv_full = q_full + 1;                   // [NST]
+  uint64_t* kv_empty = kv_full + NST;               // [NST]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&maps.q);
     tma_prefetch_desc(&maps.k);
     tma_prefetch_desc(&maps.vt);
-    for (int g = 0; g < 2; ++g) {
-      mbar_init(&q_full[g], 1); mbar_init(&q_free[g], 1);
-      mbar_init(&s_full[g], 1); mbar_init(&s_free[g], kArr);
-      mbar_init(&p_full[g], kArr); mbar_init(&o_full[g], 1); mbar_init(&o_free[g], kArr);
-    }
-    for (int s = 0; s < 4; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], NG); }
+    mbar_init(q_full, 1);
+    for (int s = 0; s < NST; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], CF::kConsumerWarps); }
     fence_mbar_init();
   }
-  if (warp == 1) { tmem_alloc(tmem_slot, 512); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();                              // prologue done: wait for the QKV kernel's q / k / v^T
+  const int bh = static_cast<int>(blockIdx.x / args.qtiles);
+  const int q0 = args.q_begin + static_cast<int>(blockIdx.x - static_cast<long long>(bh) * args.qtiles) * 128;
   const int J = args.nchunks;
   const int tail_valid = args.ntok - (J - 1) * 128;          // valid keys of the last chunk, 1..128
-  const int tail_n = (tail_valid + 15) & ~15;                // MMA width of the last chunk (N of S, K of PV)
 
-  if (warp == 0) {
+  if (warp == CF::kConsumerWarps) {
     // ===================== TMA producer =====================
     if (elect_one()) {
+      mbar_expect_tx(q_full, CF::kQBytes);
+      for (int kb = 0; kb < KB; ++kb) tma_load_3d(sQ + kb * (128 * 128), &maps.q, q_full, kb * 64, q0, bh);
       int stage = 0;
-      uint32_t kv_phase = 0;
-      uint32_t qfree_cnt[2] = {0, 0};
-      for (long long item = blockIdx.x; item < args.items; item += gridDim.x) {
-        const ItemDec d = decode_item<NG>(item, args);
-        for (int g = 0; g < d.nq; ++g) {
-          const int q0 = args.q_begin + (d.pair * NG + g) * 128;
-          mbar_wait(&q_free[g], (qfree_cnt[g] & 1) ^ 1);
-          ++qfree_cnt[g];
-          mbar_expect_tx(&q_full[g], CF::kQBytes);
-          for (int kb = 0; kb < KB; ++kb)
-            tma_load_3d(sQ + g * CF::kQBytes + kb * (128 * 128), &maps.q, &q_full[g], kb * 64, q0, d.bh);
-        }
-        for (int j = 0; j < J; ++j) {
-          mbar_wait(&kv_empty[stage], kv_phase ^ 1);
-          mbar_expect_tx(&kv_full[stage], CF::kKBytes + CF::kVBytes);
-          for (int kb = 0; kb < KB; ++kb)
-            tma_load_3d(sK + stage * CF::kKBytes + kb * (128 * 128), &maps.k, &kv_full[stage], kb * 64, j * 128, d.bh);
-          tma_load_3d(sV + stage * CF::kVBytes, &maps.vt, &kv_full[stage], j * 128, 0, d.bh);
-          tma_load_3d(sV + stage * CF::kVBytes + HD * 128, &maps.vt, &kv_full[stage], j * 128 + 64, 0, d.bh);
-          if (++stage == NST) { stage = 0; kv_phase ^= 1; }
-        }
+      uint32_t phase = 0;
+      for (int j = 0; j < J; ++j) {
+        mbar_wait(&kv_empty[stage], phase ^ 1);
+        mbar_expect_tx(&kv_full[stage], CF::kKBytes + CF::kVBytes);
+        for (int kb = 0; kb < KB; ++kb)
+          tma_load_3d(sK + stage * CF::kKBytes + kb * (128 * 128), &maps.k, &kv_full[stage], kb * 64, j * 128, bh);
+        tma_load_3d(sV + stage * CF::kVBytes, &maps.vt, &kv_full[stage], j * 128, 0, bh);
+        tma_load_3d(sV + stage * CF::kVBytes + HD * 128, &maps.vt, &kv_full[stage], j * 128 + 64, 0, bh);
+        if (++stage == NST) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp <= NG) {
-    // ===================== MMA issuer of group g (one thread per group, warps 1 and 2) =====================
-    // In-order stream per group: S(0), then per chunk j: S(j+1) (its conditions - K chunk j+1 landed, S(j) read by the
-    // softmax warps - come true before P(j) is complete), PV(j).  (A single thread polling both groups added its polling
-    // period to every hand-over.)
-    if (elect_one()) {
-      const int g = warp - 1;
-      constexpr uint32_t idesc_s = make_idesc_f16(TT::kFmt, 128, 128);
-      constexpr uint32_t idesc_o = make_idesc_f16(TT::kFmt, 128, HD);
-      const uint32_t idesc_s_tail = make_idesc_f16(TT::kFmt, 128, tail_n);
-      const uint32_t tS = tmem_base + g * CF::kGroupCols;
-      int st_s = 0, st_p = 0;                 // ring position of the next S chunk / the next PV chunk
-      uint32_t ph_s = 0, ph_p = 0;
-      uint32_t n_s = 0, n_p = 0, n_items = 0, qcnt = 0;
-      auto issue_s = [&](bool last) {
-        mbar_wait(&kv_full[st_s], ph_s);
-        mbar_wait(&s_free[g], (n_s & 1) ^ 1);                // the softmax warps have read the previous S
-        ++n_s;
-        tc_fence_after();
-        const uint32_t idesc = last ? idesc_s_tail : idesc_s;
-#pragma unroll
-        for (int kb = 0; kb < KB; ++kb) {
-          const uint64_t da = make_desc_k128(smem_u32(sQ + g * CF::kQBytes + kb * (128 * 128)));
-          const uint64_t db = make_desc_k128(smem_u32(sK + st_s * CF::kKBytes + kb * (128 * 128)));
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            tc_mma_f16(tS, da + static_cast<uint64_t>(k * 2), db + static_cast<uint64_t>(k * 2), idesc, (kb | k) != 0 ? 1u : 0u);
-        }
-        tc_commit(&s_full[g]);
-        if (last) tc_commit(&q_free[g]);                     // no later MMA of this item reads Q
-        if (++st_s == NST) { st_s = 0; ph_s ^= 1; }
-      };
-      for (long long item = blockIdx.x; item < args.items; item += gridDim.x) {
-        const ItemDec d = decode_item<NG>(item, args);
-        if (g >= d.nq) {
-          // this group sits the item out, but the K/V ring counts one release per group and stage
-          for (int j = 0; j < J; ++j) {
-            mbar_wait(&kv_full[st_p], ph_p);
-            tc_commit(&kv_empty[st_p]);
-            if (++st_p == NST) { st_p = 0; ph_p ^= 1; }
-          }
-          st_s = st_p; ph_s = ph_p;
-          continue;
-        }
-        mbar_wait(&q_full[g], qcnt & 1);
-        ++qcnt;
-        issue_s(J == 1);
-        for (int j = 0; j < J; ++j) {
-          if (j + 1 < J) issue_s(j + 2 == J);
-          mbar_wait(&p_full[g], n_p & 1);                    // P_g(j) is in smem
-          ++n_p;
-          if (j == 0) mbar_wait(&o_free[g], (n_items & 1) ^ 1);   // the previous item's O has been read out
-          tc_fence_after();
-          const int nk = (j + 1 == J) ? (tail_n >> 4) : 8;    // K = 16 steps of this chunk
-          for (int t = 0; t < nk; ++t) {
-            const int kb = t >> 2, k = t & 3;
-            const uint64_t db = make_desc_k128(smem_u32(sV + st_p * CF::kVBytes + kb * HD * 128));
-            if constexpr (PT) {
-              // A = P from tensor memory (8 columns per K = 16 step): the PV MMA reads only V^T from shared memory, whose
-              // bandwidth (128 B/clk) otherwise caps a 128 x HD x 16 MMA with a 4 KB smem A operand at 2/3 of its rate
-              tc_mma_f16_ts(tS + 128, tS + 128 + HD + t * 8, db + static_cast<uint64_t>(k * 2), idesc_o, (j | t) != 0 ? 1u : 0u);
-            } else {
-              const uint64_t da = make_desc_k128(smem_u32(sP + g * CF::kPBytes + kb * 128 * 128));
-              tc_mma_f16(tS + 128, da + static_cast<uint64_t>(k * 2), db + static_cast<uint64_t>(k * 2), idesc_o, (j | t) != 0 ? 1u : 0u);
-            }
-          }
-          tc_commit(&o_full[g]);
-          tc_commit(&kv_empty[st_p]);
-          if (++st_p == NST) { st_p = 0; ph_p ^= 1; }
-        }
-        ++n_items;
-      }
-    }
-  } else if (warp >= CF::kCtrlWarps) {
-    // ===================== softmax / output warps =====================
-    const int set = (warp - CF::kCtrlWarps) >> 2;
-    const int g = set / SPLIT;              // query tile of the pair
-    const int part = set % SPLIT;           // column / head-dim slice of this warp
-    const int q4 = warp & 3;                // TMEM lane quarter this warp may access
-    const int row = q4 * 32 + lane;
-    constexpr int CW = 128 / SPLIT;         // score columns per warp (64)
-    constexpr int OW = HD / SPLIT;          // O columns (head dims) per warp
-    const uint32_t tS = tmem_base + g * CF::kGroupCols + (static_cast<uint32_t>(q4 * 32) << 16) + part * CW;
-    const uint32_t tO = tmem_base + g * CF::kGroupCols + 128 + (static_cast<uint32_t>(q4 * 32) << 16) + part * OW;
-    const uint32_t tP = tmem_base + g * CF::kGroupCols + 128 + HD + (static_cast<uint32_t>(q4 * 32) << 16);
-    const uint32_t sP_row = smem_u32(sP + g * CF::kPBytes) + row * 128;
-    const uint32_t sP_base = smem_u32(sP + g * CF::kPBytes);
-    float* xm = xchg + (g * 128 + row) * 4;  // [2 buffers][2 parts] row maxima; the l exchange reuses the slots
-    auto pair_sync = [&]() { asm volatile("bar.sync %0, %1;" ::"r"(1 + g * 4 + q4), "n"(32 * SPLIT) : "memory"); };
-    uint32_t sfull_cnt = 0, ofull_cnt = 0;
+  } else {
+    // ===================== consumer warpgroups =====================
+    const int wg = warp >> 2;
     const float sl2 = args.scale_log2e;
-    for (long long item = blockIdx.x; item < args.items; item += gridDim.x) {
-      const ItemDec d = decode_item<NG>(item, args);
-      if (g >= d.nq) continue;              // this group has no query tile in this item (warp-uniform)
-      const int q0 = args.q_begin + (d.pair * NG + g) * 128;
-      const bool dead = q0 + q4 * 32 >= args.ntok;   // none of this warp's 32 rows exists: barrier protocol only
-      if (dead) {
-        // keep the barrier protocol in lock step (arrival counts include every warp of the group), touch no data; the
-        // P rows of these query rows hold garbage, which only reaches O rows that are never stored
-        for (int j = 0; j < J; ++j) {
-          mbar_wait(&s_full[g], sfull_cnt & 1);
-          ++sfull_cnt;
-          if (lane == 0) mbar_arrive(&s_free[g]);
-          if (j > 0) { mbar_wait(&o_full[g], ofull_cnt & 1); ++ofull_cnt; }
-          if (lane == 0) mbar_arrive(&p_full[g]);
-        }
-        mbar_wait(&o_full[g], ofull_cnt & 1);
-        ++ofull_cnt;
-        if (lane == 0) mbar_arrive(&o_free[g]);
-        continue;
+    float o[HD / 2];
+#pragma unroll
+    for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
+    float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;   // rows lane/4 and lane/4 + 8 of this warp's 16
+    mbar_wait(q_full, 0);
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int j = 0; j < J; ++j) {
+      const int lim = j + 1 == J ? tail_valid : 128;       // valid keys of this chunk
+      mbar_wait(&kv_full[stage], phase);
+      float s[64];
+      wgmma_fence();
+#pragma unroll
+      for (int kb = 0; kb < KB; ++kb) {
+        const uint64_t da = make_gdesc_k128(smem_u32(sQ + kb * (128 * 128) + wg * 64 * 128));
+        const uint64_t db = make_gdesc_k128(smem_u32(sK + stage * CF::kKBytes + kb * (128 * 128)));
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          wgmma_ss<TT::kFmt, 128>(s, da + static_cast<uint64_t>(k * 2), db + static_cast<uint64_t>(k * 2), (kb | k) != 0 ? 1u : 0u);
       }
-      float m = -INFINITY, l = 0.f;
-      SmCtx cx;
-      cx.tS = tS; cx.tO = tO; cx.tP = tP; cx.sP_row = sP_row; cx.row = row; cx.part = part; cx.lane = lane; cx.xm = xm; cx.sl2 = sl2;
-      cx.s_full = &s_full[g]; cx.s_free = &s_free[g]; cx.p_full = &p_full[g]; cx.o_full = &o_full[g];
-      cx.bar_id = 1 + g * 4 + q4;
-      for (int j = 0; j + 1 < J; ++j) softmax_chunk<TT, HD, false, kOne, POLY, PT>(cx, j, 2, 64, m, l, sfull_cnt, ofull_cnt);
-      {
-        int ngrp = (tail_n - part * CW + 31) >> 5;             // 32-column groups this warp owns in the last chunk
-        ngrp = ngrp < 0 ? 0 : (ngrp > CW / 32 ? CW / 32 : ngrp);
-        softmax_chunk<TT, HD, true, kOne, POLY, PT>(cx, J - 1, ngrp, tail_valid - part * CW, m, l, sfull_cnt, ofull_cnt);
+      wgmma_commit();
+      wgmma_wait<0>();
+      // ---- online softmax.  s[4c + {0,1}]: row 0, keys 8c + 2(lane%4) + {0,1}; s[4c + {2,3}]: row 1, same keys
+#pragma unroll
+      for (int c = 0; c < 16; ++c) {                        // selects, not branches
+        const int key = 8 * c + 2 * (lane & 3);
+        s[4 * c] = key < lim ? s[4 * c] : -INFINITY;
+        s[4 * c + 2] = key < lim ? s[4 * c + 2] : -INFINITY;
+        s[4 * c + 1] = key + 1 < lim ? s[4 * c + 1] : -INFINITY;
+        s[4 * c + 3] = key + 1 < lim ? s[4 * c + 3] : -INFINITY;
       }
-      // ---- last PV retired: read this warp's O slice, release the accumulator for the next item
-      mbar_wait(&o_full[g], ofull_cnt & 1);
-      ++ofull_cnt;
-      tc_fence_after();
-      uint32_t o[OW / 32][32];
+      float mx0 = -INFINITY, mx1 = -INFINITY;
 #pragma unroll
-      for (int h = 0; h < OW / 32; ++h) tmem_ld32(tO + h * 32, o[h]);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&o_free[g]);
-      // ---- row sums of the column slices add up (same reference maximum in both warps of the row)
-      pair_sync();                                   // the partner has consumed the last row-max slots
-      xm[part] = l;
-      pair_sync();
-      l += xm[part ^ 1];
-      // ---- normalise, stage this warp's head dims of its 32 rows through (now free) P smem (64 dims per 16 KB block)
-      const float inv = 1.f / l;
-      __syncwarp();
-#pragma unroll
-      for (int c = 0; c < OW / 8; ++c) {
-        const int dim0 = part * OW + 8 * c;          // first head dim of this 16-byte chunk
-#define B2U_O(k_) (__uint_as_float(o[(8 * c + (k_)) >> 5][(8 * c + (k_)) & 31]) * inv)
-        sts128a(sP_row + (dim0 >> 6) * (128 * 128) + ((((dim0 >> 3) & 7) ^ (row & 7)) << 4), TT::pack2(B2U_O(0), B2U_O(1)),
-                TT::pack2(B2U_O(2), B2U_O(3)), TT::pack2(B2U_O(4), B2U_O(5)), TT::pack2(B2U_O(6), B2U_O(7)));
-#undef B2U_O
+      for (int c = 0; c < 16; ++c) {
+        mx0 = fmaxf(mx0, fmaxf(s[4 * c], s[4 * c + 1]));
+        mx1 = fmaxf(mx1, fmaxf(s[4 * c + 2], s[4 * c + 3]));
       }
-      __syncwarp();
-      pair_sync();                                   // both dim slices of these 32 rows are staged
-      const int b = d.bh / args.heads, hd = d.bh - b * args.heads;
-      const int D = args.heads * HD;
-      T* outp = reinterpret_cast<T*>(args.out);
+      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
+      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
+      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+      const float mn0 = fmaxf(m0, mx0 * sl2), mn1 = fmaxf(m1, mx1 * sl2);   // chunk 0 always has valid keys -> finite
+      const float corr0 = ex2(m0 - mn0), corr1 = ex2(m1 - mn1);             // 0 on the first chunk
+      m0 = mn0;
+      m1 = mn1;
+      float rs0 = 0.f, rs1 = 0.f;
+      uint32_t pa[8][4];                                    // P as the A fragments of the 8 K = 16 steps
 #pragma unroll
-      for (int hb = 0; hb < HD / 64; ++hb)
+      for (int c = 0; c < 16; ++c) {
+        const float p0 = ex2(fmaf(s[4 * c], sl2, -mn0)), p1 = ex2(fmaf(s[4 * c + 1], sl2, -mn0));
+        const float p2 = ex2(fmaf(s[4 * c + 2], sl2, -mn1)), p3 = ex2(fmaf(s[4 * c + 3], sl2, -mn1));
+        rs0 += p0 + p1;
+        rs1 += p2 + p3;
+        pa[c >> 1][(c & 1) * 2] = TT::pack2(p0, p1);
+        pa[c >> 1][(c & 1) * 2 + 1] = TT::pack2(p2, p3);
+      }
+      l0 = l0 * corr0 + rs0;                                // per-lane partial sums of the un-rounded probabilities
+      l1 = l1 * corr1 + rs1;
 #pragma unroll
-        for (int ii = 0; ii < 8 / SPLIT; ++ii) {     // the warps of a row quarter split its 32 rows
-          const int i = part * (8 / SPLIT) + ii;
-          const int rr = q4 * 32 + i * 4 + (lane >> 3);
-          const uint4 val = lds128a(sP_base + hb * (128 * 128) + rr * 128 + (((lane & 7) ^ (rr & 7)) << 4));
-          const int t = q0 + rr;
-          if (t < args.ntok)
-            *reinterpret_cast<uint4*>(outp + (static_cast<long long>(b) * args.ntok + t) * D + hd * HD + hb * 64 + (lane & 7) * 8) = val;
-        }
-      __syncwarp();
-      pair_sync();                                   // the partner has read my staged chunks: P smem may be rewritten
+      for (int c = 0; c < HD / 8; ++c) {
+        o[4 * c] *= corr0; o[4 * c + 1] *= corr0;
+        o[4 * c + 2] *= corr1; o[4 * c + 3] *= corr1;
+      }
+      // ---- O += P V_j
+      wgmma_fence();
+#pragma unroll
+      for (int t = 0; t < 8; ++t) {
+        const uint64_t db = make_gdesc_k128(smem_u32(sV + stage * CF::kVBytes + (t >> 2) * (HD * 128)));
+        wgmma_rs<TT::kFmt, HD>(o, pa[t], db + static_cast<uint64_t>((t & 3) * 2), 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      if (lane == 0) mbar_arrive(&kv_empty[stage]);
+      if (++stage == NST) { stage = 0; phase ^= 1; }
+    }
+    // ---- normalise and store: rows q0 + 64 wg + 16 (warp % 4) + lane / 4 (+ 8), head dims 8c + 2 (lane % 4) + {0, 1}
+    l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+    l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+    const float inv0 = 1.f / l0, inv1 = 1.f / l1;
+    const int b = bh / args.heads, hd = bh - b * args.heads;
+    const int D = args.heads * HD;
+    const int t0 = q0 + wg * 64 + (warp & 3) * 16 + (lane >> 2), t1 = t0 + 8;
+    T* outp = reinterpret_cast<T*>(args.out) + static_cast<long long>(b) * args.ntok * D + hd * HD + 2 * (lane & 3);
+#pragma unroll
+    for (int c = 0; c < HD / 8; ++c) {
+      if (t0 < args.ntok)
+        *reinterpret_cast<uint32_t*>(outp + static_cast<long long>(t0) * D + 8 * c) = TT::pack2(o[4 * c] * inv0, o[4 * c + 1] * inv0);
+      if (t1 < args.ntok)
+        *reinterpret_cast<uint32_t*>(outp + static_cast<long long>(t1) * D + 8 * c) = TT::pack2(o[4 * c + 2] * inv1, o[4 * c + 3] * inv1);
     }
   }
-  pdl_launch_dependents();   // this CTA's items are done
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
+  pdl_launch_dependents();   // this CTA's rows are done
 }
 
-template <typename T, int HD, bool kOne, int POLY, bool PT = false>
+template <typename T, int HD>
 static int launch_attn_tc3(const AttnMaps& maps, const AttnArgs& a, cudaStream_t stream) {
-  auto kern = attn_tc3_kernel<T, HD, kOne, POLY, PT>;
-  using CF = At3Cfg<HD>;
+  auto kern = attn_tc3_kernel<T, HD>;
+  using CF = AttCfg<HD>;
   static_assert(CF::kSmem <= 227 * 1024, "attention smem budget");
   static bool configured_dev[64] = {};
   bool& configured = configured_dev[current_device_index()];
@@ -536,26 +193,15 @@ static int launch_attn_tc3(const AttnMaps& maps, const AttnArgs& a, cudaStream_t
     if (e != cudaSuccess) return set_error(-2, "cudaFuncSetAttribute(attn_tc3): %s", cudaGetErrorString(e));
     configured = true;
   }
-  const int sms = num_sms();
-  const int grid = static_cast<int>(a.items < sms ? a.items : sms);
-  launch_pdl(kern, grid, CF::kThreads, CF::kSmem, stream, maps, a);
+  if (a.items > 0x7fffffffLL) return set_error(-1, "b2u_attention_tc: too many query tiles");
+  launch_pdl(kern, static_cast<int>(a.items), CF::kThreads, CF::kSmem, stream, maps, a);
   return check_launch("attention_tc3");
 }
 
-int attention_tc3_dispatch(const AttnMaps& maps, const AttnArgs& a, int head_dim, int dtype, int variant, cudaStream_t stream) {
-  // variant (b2u_set_option(4, .)): 0 = default (P in tensor memory), 8 = P through shared memory (round-2 first version), 4 = single-pass softmax, 6 = every exp2 on the MUFU pipe, 7 = every 4th exp2 on the FMA pipe (default: every 3rd; measured: 1/2 and packed-pair polynomials lose)
+int attention_tc3_dispatch(const AttnMaps& maps, const AttnArgs& a, int head_dim, int dtype, cudaStream_t stream) {
   const bool bf = dtype == B2U_BF16;
-  if (head_dim == 64) {
-    if (variant == 4) return bf ? launch_attn_tc3<__nv_bfloat16, 64, true, 0>(maps, a, stream) : launch_attn_tc3<__half, 64, true, 0>(maps, a, stream);
-    if (variant == 6) return bf ? launch_attn_tc3<__nv_bfloat16, 64, false, 0>(maps, a, stream) : launch_attn_tc3<__half, 64, false, 0>(maps, a, stream);
-    if (variant == 7) return bf ? launch_attn_tc3<__nv_bfloat16, 64, false, 4>(maps, a, stream) : launch_attn_tc3<__half, 64, false, 4>(maps, a, stream);
-    if (variant == 8) return bf ? launch_attn_tc3<__nv_bfloat16, 64, false, 3>(maps, a, stream) : launch_attn_tc3<__half, 64, false, 3>(maps, a, stream);
-    return bf ? launch_attn_tc3<__nv_bfloat16, 64, false, 3, true>(maps, a, stream) : launch_attn_tc3<__half, 64, false, 3, true>(maps, a, stream);
-  }
-  // head_dim 128: 320 threads compile to 168 registers -> the single-pass softmax fits without spills; exp2 is half as
-  // dense per flop there, MUFU is not the limiter
-  if (variant == 8) return bf ? launch_attn_tc3<__nv_bfloat16, 128, true, 0>(maps, a, stream) : launch_attn_tc3<__half, 128, true, 0>(maps, a, stream);
-  return bf ? launch_attn_tc3<__nv_bfloat16, 128, true, 0, true>(maps, a, stream) : launch_attn_tc3<__half, 128, true, 0, true>(maps, a, stream);
+  if (head_dim == 64) return bf ? launch_attn_tc3<__nv_bfloat16, 64>(maps, a, stream) : launch_attn_tc3<__half, 64>(maps, a, stream);
+  return bf ? launch_attn_tc3<__nv_bfloat16, 128>(maps, a, stream) : launch_attn_tc3<__half, 128>(maps, a, stream);
 }
 
 }  // namespace b2u

@@ -1,4 +1,4 @@
-"""Builds libdinounet_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Builds libdinounet_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU)."""
 import os
 import subprocess
 import sys
@@ -11,7 +11,8 @@ SUFFIX = os.environ.get("B2U_OUT_SUFFIX", "")
 EXTRA = os.environ.get("B2U_EXTRA_FLAGS", "").split()
 OUT = os.path.join(os.path.dirname(HERE), f"libdinounet_b200{SUFFIX}.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = [*ARCH, "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "--use_fast_math=false"]
 FLAGS = [f for f in FLAGS if not f.startswith("--use_fast_math")]
 
@@ -20,7 +21,7 @@ def _stale(obj, src):
     if not os.path.exists(obj):
         return True
     t = os.path.getmtime(obj)
-    deps = [src] + [os.path.join(HERE, f) for f in os.listdir(HERE) if f.endswith((".cuh", ".h"))]
+    deps = [src, __file__] + [os.path.join(HERE, f) for f in os.listdir(HERE) if f.endswith((".cuh", ".h"))]
     deps.append(os.path.join(HERE, "..", "..", "include", "dinounet_b200.h"))
     return any(os.path.getmtime(d) > t for d in deps)
 
@@ -51,7 +52,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         if verbose and out.strip():
             print(out)
     if relink:
-        cmd = [NVCC, "-shared", "-o", OUT, *objs, "-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = [NVCC, "-shared", "-o", OUT, *objs, *ARCH]
         r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}")

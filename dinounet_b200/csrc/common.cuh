@@ -1,4 +1,4 @@
-// Common device helpers for the sm_100a kernels: mbarrier / TMA / tcgen05 PTX wrappers, 16-bit type traits.
+// Common device helpers for the sm_90a kernels: mbarrier / TMA PTX wrappers, 16-bit type traits.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -11,7 +11,7 @@ namespace b2u {
 // ---------------------------------------------------------------- 16-bit element traits
 template <typename T> struct T16;
 template <> struct T16<__nv_bfloat16> {
-  static constexpr int kFmt = 1;  // tcgen05 instr-desc a/b format: 1 = BF16
+  static constexpr int kFmt = 1;  // = B2U_BF16 (wgmma_ss / wgmma_rs kind)
   __device__ static __forceinline__ float to_f(__nv_bfloat16 v) { return __bfloat162float(v); }
   __device__ static __forceinline__ __nv_bfloat16 from_f(float v) { return __float2bfloat16_rn(v); }
   __device__ static __forceinline__ uint32_t pack2(float a, float b) {
@@ -24,7 +24,7 @@ template <> struct T16<__nv_bfloat16> {
   }
 };
 template <> struct T16<__half> {
-  static constexpr int kFmt = 0;  // 0 = F16
+  static constexpr int kFmt = 0;  // = B2U_F16
   __device__ static __forceinline__ float to_f(__half v) { return __half2float(v); }
   __device__ static __forceinline__ __half from_f(float v) { return __float2half_rn(v); }
   __device__ static __forceinline__ uint32_t pack2(float a, float b) {
@@ -100,9 +100,8 @@ __device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
 }
 
 // One elected lane of a fully converged warp (PTX elect.sync).  Unlike `lane == 0`, the compiler KNOWS that exactly one
-// thread executes the guarded region, so uniform-datapath instructions (UTCHMMA, UTMALDG, UTCBAR) are emitted straight
-// instead of inside an ELECT / BRA.U.ANY waterfall loop each (about 8 extra SASS instructions per tcgen05.mma, which made
-// the single MMA-issuer thread the bottleneck of the small-N convolution tiles).
+// thread executes the guarded region, so uniform-datapath instructions (UTMALDG) are emitted straight instead of inside a
+// waterfall loop each.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -135,211 +134,10 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const void* map, uin
       : "memory");
 }
 
-// L2 prefetch of a 4-D tensor-map box (no shared-memory destination, no barrier): warms L2 for a later TMA load
-__device__ __forceinline__ void tma_prefetch_4d(const void* map, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.prefetch.tensor.4d.L2.global.tile [%0, {%1, %2, %3, %4}];" ::"l"(reinterpret_cast<uint64_t>(map)),
-               "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
-
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 (fp16 / bf16 inputs, fp32 accumulate)
-__device__ __forceinline__ void tc_mma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                           uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]: the A operand (M = 128 rows on the 128 lanes, K-major: two 16-bit elements per 32-bit
-// column, 8 columns per K = 16 step) is read from tensor memory
-__device__ __forceinline__ void tc_mma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread i <-> TMEM lane base+i)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---------------------------------------------------------------- CTA pairs (cluster of 2, tcgen05 cta_group::2)
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of `smem_addr` (a shared::cta address of this CTA) in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t smem_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  // default semantics (release at CTA scope): the consumer only needs "this warp's TMEM reads are done", which the
-  // tcgen05 fence before the arrive provides; a cluster-scope release would also drain this thread's global stores
-  // (MEMBAR + ERRBAR per tile, 6 % of the QKV kernel's stall samples)
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA load whose completion bytes are posted on an mbarrier that may live in the peer CTA of the pair
-__device__ __forceinline__ void tma_load_2d_pair(void* smem_dst, const void* map, uint32_t bar_cluster_addr, int c0,
-                                                 int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], "
-      "[%2];" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish2() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// commit of the pair's MMAs: arrives on the mbarrier at this smem offset in every CTA of `mask`
-__device__ __forceinline__ void tc_commit_pair(uint64_t* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::
-                   "r"(smem_u32(bar)),
-               "h"(mask)
-               : "memory");
-}
-// D[tmem of both CTAs] (+)= A[256 x 16: 128 rows from each CTA's smem] * B[N x 16: N/2 rows from each CTA's smem]
-__device__ __forceinline__ void tc_mma_f16_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// K-major, 128B-swizzled shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout):
-//   [0,14) start>>4 | [16,30) LBO>>4 (=1 for swizzled K-major) | [32,46) SBO>>4 (1024 B between 8-row groups)
-//   [46,48) version=1 | [61,64) layout type 2 = SWIZZLE_128B
-__device__ __forceinline__ uint64_t make_desc_k128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-// same, with an explicit stride between 8-row groups (a window into a wider swizzled tile: one group per tile row)
-__device__ __forceinline__ uint64_t make_desc_k128_sbo(uint32_t smem_addr, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(sbo_bytes >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-// Instruction descriptor for kind::f16, fp32 accumulate, K-major A and B (cute::UMMA::InstrDescriptor).
-__host__ __device__ constexpr uint32_t make_idesc_f16(int fmt_ab, int M, int N) {
-  return (1u << 4) | (static_cast<uint32_t>(fmt_ab) << 7) | (static_cast<uint32_t>(fmt_ab) << 10) |
-         (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
-}
-
-// packed fp32 pair arithmetic (sm_100 FFMA2 / FADD2 / FMUL2): one issue slot for two lanes
-__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
-  float2 d;
-  asm("{\n"
-      ".reg .b64 ra, rb, rc, rd;\n"
-      "mov.b64 ra, {%2, %3};\n"
-      "mov.b64 rb, {%4, %5};\n"
-      "mov.b64 rc, {%6, %7};\n"
-      "fma.rn.f32x2 rd, ra, rb, rc;\n"
-      "mov.b64 {%0, %1}, rd;\n"
-      "}\n"
-      : "=f"(d.x), "=f"(d.y)
-      : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y), "f"(c.x), "f"(c.y));
-  return d;
-}
-__device__ __forceinline__ float2 add2(float2 a, float2 b) {
-  float2 d;
-  asm("{\n"
-      ".reg .b64 ra, rb, rd;\n"
-      "mov.b64 ra, {%2, %3};\n"
-      "mov.b64 rb, {%4, %5};\n"
-      "add.rn.f32x2 rd, ra, rb;\n"
-      "mov.b64 {%0, %1}, rd;\n"
-      "}\n"
-      : "=f"(d.x), "=f"(d.y)
-      : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-  return d;
-}
-
-__device__ __forceinline__ float2 mul2(float2 a, float2 b) {
-  float2 d;
-  asm("{\n"
-      ".reg .b64 ra, rb, rd;\n"
-      "mov.b64 ra, {%2, %3};\n"
-      "mov.b64 rb, {%4, %5};\n"
-      "mul.rn.f32x2 rd, ra, rb;\n"
-      "mov.b64 {%0, %1}, rd;\n"
-      "}\n"
-      : "=f"(d.x), "=f"(d.y)
-      : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-  return d;
-}
+// fp32 pair arithmetic (two lanes of a float2; sm_90 has no packed f32x2 instructions, so each is two scalar ones)
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 

@@ -2,7 +2,7 @@
 // operator.  It exists for ONE purpose: north_star's "within 1e-5 of the reference PyTorch forward in fp32" - the
 // reference's fp32 regime is its CPU forward (autocast('cuda') self-disables, dinov3_adapter.py:422), which the 16-bit
 // tensor-core path cannot meet by construction (BASELINE.md section 5: bf16-ViT noise floor 2.5e-2).  These kernels are
-// deliberately simple (no tensor cores: tcgen05 kind::tf32 keeps 10 mantissa bits, and the bf16x3 split accumulates with
+// deliberately simple (no tensor cores: TF32 keeps 10 mantissa bits, and the bf16x3 split accumulates with
 // truncation) and are NOT the benchmarked path; `DinoUNet.precision = "fp32"` selects them.
 // Layout: tokens [rows, C] / images NHWC fp32, same as the 16-bit engine.  Weights: [N, K] K-major fp32
 // (conv: k = tap * Cpad + c), packed by ForwardEngine.pack with dtype float32.

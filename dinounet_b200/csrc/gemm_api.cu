@@ -1,5 +1,5 @@
 // Host side of the tensor-core GEMM / implicit-GEMM convolution entry points (b2u_gemm, b2u_qkv_rope): shape checks, tile
-// choice, TMA tensor maps, dispatch to the persistent tcgen05 kernel family of gemm_tc2.cu.
+// choice, TMA tensor maps, dispatch to the persistent wgmma kernel family of gemm_tc2.cu.
 #include "common.cuh"
 #include "../../include/dinounet_b200.h"
 #include "host_util.h"
@@ -7,12 +7,11 @@
 
 namespace b2u {
 
-static int pick_bn(int N, bool v2) {
+// BLOCK_N: the fp32 accumulator tile (128 x BN) and the TMA ring share the 227 KB of shared memory, so tiles stop at 128
+static int pick_bn(int N) {
   if (N <= 32) return 32;
   if (N <= 64) return 64;
-  if (!v2 || N <= 128) return 128;
-  const int waste = (N + 255) / 256 * 256 - N;
-  return (waste == 0 || waste * 8 <= N) ? 256 : 128;
+  return 128;
 }
 
 static int run_gemm(bool qkv, int bn, int dtype, const GemmMaps& maps, const GemmArgs& args, cudaStream_t stream) {
@@ -41,10 +40,9 @@ extern "C" int b2u_gemm(const b2u_gemm_params* p, b2u_stream_t stream_) {
   a.N = p->N;
   a.epi = p->epi;
   a.conv = p->conv;
-  const bool v2 = true;   // (the first-generation one-tile-per-CTA kernel was removed in round 2)
-  if (e.act1 == B2U_ACT_SWIGLU && (!v2 || p->N % 64 || p->conv != B2U_CONV_NONE))
-    return set_error(-1, "b2u_gemm: SwiGLU epilogue needs the v2 kernel, N %% 64 == 0 and a plain GEMM");
-  const int bn = (e.act1 == B2U_ACT_SWIGLU && p->N <= 128) ? 128 : pick_bn(p->N, v2);
+  if (e.act1 == B2U_ACT_SWIGLU && (p->N % 64 || p->conv != B2U_CONV_NONE))
+    return set_error(-1, "b2u_gemm: SwiGLU epilogue needs N %% 64 == 0 and a plain GEMM");
+  const int bn = e.act1 == B2U_ACT_SWIGLU ? 128 : pick_bn(p->N);
   a.n_tiles = (p->N + bn - 1) / bn;
   long long m_tiles;
   int rc;
@@ -52,11 +50,9 @@ extern "C" int b2u_gemm(const b2u_gemm_params* p, b2u_stream_t stream_) {
     a.M = p->M;
     a.num_kb = (p->K + BK - 1) / BK;
     m_tiles = (static_cast<long long>(p->M) + BM - 1) / BM;
-    // CTA pairs (cta_group::2) for the 256-wide tiles of plain GEMMs (option 3 = 1 disables, for A/B runs)
-    a.pair = (v2 && bn == 256 && m_tiles >= 2 && get_option(3) != 1) ? 1 : 0;
     a.res_prefetch = (get_option(7) != 1 && a.num_kb <= 8) ? 1 : 0;   // short K only: measured +3 % there, nothing (or worse) at K >= 1024
     if ((rc = make_map_2d(&maps.a[0], p->A, p->M, p->K, p->lda, BM, p->dtype))) return rc;
-    if ((rc = make_map_2d(&maps.b, p->Wp, p->N, p->K, p->ldw, a.pair ? bn / 2 : bn, p->dtype))) return rc;
+    if ((rc = make_map_2d(&maps.b, p->Wp, p->N, p->K, p->ldw, bn, p->dtype))) return rc;
   } else {
     const int stride = p->conv == B2U_CONV3X3_S2 ? 2 : 1;
     if (p->C % 8) return set_error(-1, "b2u_gemm(conv): C must be a multiple of 8");
@@ -76,20 +72,7 @@ extern "C" int b2u_gemm(const b2u_gemm_params* p, b2u_stream_t stream_) {
     m_tiles = static_cast<long long>(p->B) * a.tiles_x * a.tiles_y;
     a.M = p->B * a.Ho * a.Wo;
     const int64_t C = p->C;
-    // halo-reuse mode (option 2 != 0 disables): stride 1, <= 64 input channels, <= 64 output channels.
-    // One [18 rows x 10 px] halo box per 16 x 8 output tile feeds all 9 taps (1.4x instead of 9x L2 -> SM traffic).
-    const int halo_opt = get_option(2);
-    if (v2 && halo_opt != 1 && stride == 1 && p->C <= 64 && p->N <= 64 && a.Wo % 8 == 0 && a.Ho >= 16) {
-      a.conv = 3;
-      a.TW = 8; a.TH = 16; a.tiles_x = a.Wo / 8; a.tiles_y = (a.Ho + 15) / 16;
-      m_tiles = static_cast<long long>(p->B) * a.tiles_x * a.tiles_y;
-      a.halo_stages = bn <= 32 ? 6 : 5;
-      cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)p->Win, (cuuint64_t)p->Hin, (cuuint64_t)p->B};
-      cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)C * p->Win * 2, (cuuint64_t)C * p->Win * p->Hin * 2};
-      cuuint32_t box[4] = {BK, 10, 18, 1};
-      cuuint32_t estr[4] = {1, 1, 1, 1};
-      if ((rc = encode_tensor_map(&maps.a[0], p->dtype, 4, p->A, dims, strides, box, estr))) return rc;
-    } else if (stride == 1) {
+    if (stride == 1) {
       cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)p->Win, (cuuint64_t)p->Hin, (cuuint64_t)p->B};
       cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)C * p->Win * 2, (cuuint64_t)C * p->Win * p->Hin * 2};
       cuuint32_t box[4] = {BK, (cuuint32_t)a.TW, (cuuint32_t)a.TH, 1};
@@ -124,17 +107,15 @@ extern "C" int b2u_qkv_rope(const b2u_qkv_params* p, b2u_stream_t stream_) {
   a.M = p->B * p->ntok;
   a.N = 3 * p->D;
   a.num_kb = (p->D + BK - 1) / BK;
-  const bool v2 = true;   // (the first-generation one-tile-per-CTA kernel was removed in round 2)
-  const int bn = v2 ? pick_bn(a.N, true) : 128;
+  const int bn = pick_bn(a.N);
   a.n_tiles = (a.N + bn - 1) / bn;
   a.conv = 0;
   a.epi.bias = p->bias;
   a.ntok = p->ntok; a.D = p->D; a.heads = p->heads; a.prefix = p->prefix; a.head_dim = head_dim;
-  if (head_dim == 128 && !v2) return set_error(-1, "b2u_qkv_rope: head_dim 128 needs the v2 GEMM kernel");
   a.rope_sin = p->rope_sin; a.rope_cos = p->rope_cos;
   a.q = p->q; a.k = p->k; a.v = p->v;
   a.npad = p->v_transposed ? p->npad : 0;
-  if (p->rope_w > 0 && v2) {
+  if (p->rope_w > 0) {
     a.rope_w = p->rope_w;
     a.rope_h = (p->ntok - p->prefix) / p->rope_w;
     if (a.rope_h * a.rope_w != p->ntok - p->prefix || (a.rope_h + a.rope_w) * (head_dim * 2 + 16) > 128 * 32 * 2 * 4)
@@ -143,10 +124,8 @@ extern "C" int b2u_qkv_rope(const b2u_qkv_params* p, b2u_stream_t stream_) {
   if (a.npad && (a.npad % 8 || a.npad < p->ntok)) return set_error(-1, "b2u_qkv_rope: bad npad");
   int rc;
   a.m_tiles = static_cast<int>((static_cast<long long>(a.M) + BM - 1) / BM);
-  a.pair = (v2 && bn == 256 && a.m_tiles >= 2 && get_option(3) != 1) ? 1 : 0;
   if ((rc = make_map_2d(&maps.a[0], p->A, a.M, p->D, p->lda, BM, p->dtype))) return rc;
-  if ((rc = make_map_2d(&maps.b, p->Wp, a.N, p->D, p->ldw, a.pair ? bn / 2 : bn, p->dtype))) return rc;
-  if (a.npad && !v2) return set_error(-1, "b2u_qkv_rope: V^T output needs the v2 GEMM kernel");
+  if ((rc = make_map_2d(&maps.b, p->Wp, a.N, p->D, p->ldw, bn, p->dtype))) return rc;
   return run_gemm(true, bn, p->dtype, maps, a, stream);
 }
 

@@ -1,4 +1,4 @@
-// Shared between the GEMM host API (gemm_api.cu) and the persistent tcgen05 kernel family (gemm_tc2.cu).
+// Shared between the GEMM host API (gemm_api.cu) and the persistent wgmma kernel family (gemm_tc2.cu).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -34,8 +34,6 @@ struct GemmArgs {
   void* v;
   int npad;  // > 0: V is written transposed as V^T [B, heads, 64, npad]
   int rope_h, rope_w;  // > 0: separable rope tables staged in smem
-  int halo_stages;  // conv == 3 (halo-reuse 3x3 mode)
-  int pair;         // 1: CTA-pair (tcgen05 cta_group::2) kernel, W map box holds BLOCK_N / 2 rows
   int res_prefetch; // 1: the epilogue pulls the NEXT tile's residual rows into L2 while it drains the current tile
 };
 

@@ -1,60 +1,60 @@
-// tcgen05 GEMM / implicit-GEMM 3x3 convolution, v2: persistent, warp-specialised, double-buffered TMEM.
+// Warp-specialised persistent GEMM / implicit-GEMM 3x3 convolution on the sm_90a warpgroup MMA (wgmma), fp16 / bf16
+// operands, fp32 accumulation.
 //
-//   grid = min(#tiles, #SMs) CTAs of 320 threads, one per SM, each looping over output tiles (n fastest, so the CTAs
-//   running concurrently share A rows through L2):
-//     warp 0   : TMA producer  — 4-stage (BN<=128: 6-stage) ring of {A 128x64, W BNx64} 128B-swizzled tiles
-//     warp 1   : MMA issuer    — one thread issues tcgen05.mma (M=128, N=BN, K=16) into accumulator buffer (tile & 1)
-//     warps 2-9: epilogue      — two warps per 32-lane TMEM quarter (each takes half of the tile's columns):
-//                                tcgen05.ld in 32-column chunks, transpose through a
-//                                swizzled 4 KB smem patch per warp, then apply the fused epilogue in a row-contiguous
-//                                layout (per-column params are per-lane constants) and issue fully coalesced 16 B
-//                                loads/stores (residual / skip tensors / output).
-//   The accumulator of tile i+1 is produced while the epilogue drains tile i (TMEM: 2 x BN columns).
-//   PAIR variants (256-wide tiles of plain GEMMs): the scheduling unit is a cluster of two CTAs that issues
-//   tcgen05.mma.cta_group::2 (M = 256); each CTA stages its own 128 A rows and HALF of the W tile, both post their TMA
-//   bytes on the leader's mbarrier, commits are multicast to both CTAs, each CTA drains its own 128 accumulator rows.
-//   Convolution mode: A tiles are 4-D TMA halo boxes of the NHWC image (9 taps x channel blocks, OOB = zero padding).
+//   grid = min(#tiles, #SMs) CTAs of 288 threads, one per SM, each looping over 128 x BN output tiles (n fastest, so the
+//   CTAs running concurrently share A rows through L2):
+//     warp 8     : TMA producer - a ring of {A 128x64, W BNx64} 128B-swizzled k-blocks (as many stages as shared memory
+//                  holds next to the accumulator tile: 3-8)
+//     warps 0-7  : two consumer warpgroups, 64 tile rows each: wgmma m64nBNk16 straight from the ring (one k-block stays in
+//                  flight while the previous stage is released), then the accumulator fragments go to a row-major fp32
+//                  tile in shared memory and the same eight warps run the fused epilogue on it with one thread per tile
+//                  row: per-column parameters are per-lane constants, and a swizzled 4 KB patch per warp transposes the
+//                  result for fully coalesced 16 B loads / stores (residual / skip tensors / output).
+//   The producer streams the next tile's k-blocks while the epilogue drains the current one.
+//   Convolution mode: A tiles are 4-D TMA boxes of the NHWC image (9 taps x channel blocks, OOB = zero padding).
 #include "common.cuh"
 #include "../../include/dinounet_b200.h"
 #include "host_util.h"
 #include "gemm_common.h"
+#include "wgmma.cuh"
 
 namespace b2u {
 
-// Halo-reuse 3x3 mode: an output tile is 16 rows x 8 pixels (= 128 MMA rows); ONE TMA box of 18 rows x 10 px x 64 ch feeds
-// all 9 taps.  Read amplification L2 -> SM is 180 / 128 = 1.4x.  (Round 1 used 1 row x 128 px tiles with a 3 x 130 halo:
-// 3.05x, and ncu showed that kernel bound by exactly that L2 -> SM traffic: 40 % of the stall samples were the epilogue
-// warps waiting for an accumulator, L2 hit rate 57 %, DRAM 26 %.)  The A operand of tap (dy, dx) is the shifted window
-// starting at halo pixel (dy, dx): 16 groups of 8 consecutive pixels, group stride = one halo row = 10 x 128 B - which is
-// what the descriptor's stride-byte-offset expresses (1280 instead of the dense 1024).
-constexpr int kHaloW = 10;                             // 8 output pixels + 1 halo pixel on each side
-constexpr int kHaloH = 18;                             // 16 output rows + 1 halo row above and below
-constexpr int kHaloBytes = kHaloH * kHaloW * 128;      // one TMA box: 18 rows x 10 px x 64 ch x 2 B = 23040 B
-constexpr int kHaloStageBytes = 23 * 1024;             // box rounded up to the 1024 B swizzle period
-constexpr int kHaloPrefetch = 8;                       // L2 prefetch distance of the halo boxes, in tiles of one CTA
-
 constexpr int kRopeBytes = 128 * 32 * 2 * 4;   // (rope_h + rope_w) rows x (<=32 angles x {sin, cos} fp32 + 16 B pad): host-checked
+constexpr int kSmemMax = 227 * 1024;           // dynamic shared memory of one CTA on sm_90
 
-// PAIR: two CTAs of a cluster form one tcgen05 cta_group::2 unit: a 256 x BN output tile, each CTA stages its own 128
-// rows of A and HALF of the W tile (BN/2 rows), so a stage is A 16 KB + W 16 KB (BN 256) instead of 16 + 32 KB: 1.5x less
-// L2 -> SM traffic per flop and a 1.5x deeper TMA ring in the same shared memory.
-template <int BN, int EPI = 0, bool PAIR = false> struct Cfg2 {
-  // the QKV variant trades pipeline stages for the in-smem rope tables
-  static constexpr int kStages = PAIR ? ((BN == 256) ? (EPI == 2 ? 5 : 6) : 8)
-                                      : ((BN == 256) ? (EPI == 2 ? 3 : 4) : (BN == 128 ? (EPI == 2 ? 5 : 6) : 8));
+template <int BN, int EPI = 0> struct Cfg2 {
   static constexpr int kABytes = BM * BK * 2;
-  static constexpr int kBBytes = (PAIR ? BN / 2 : BN) * BK * 2;
+  static constexpr int kBBytes = BN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kEpiWarps = (EPI == 4 || (EPI == 2 && BN == 256)) ? 16 : 8;   // latency-bound GELU / RoPE epilogues: four warps per TMEM lane quarter
-  static constexpr int kThreads = 64 + 32 * kEpiWarps;  // producer warp + MMA warp + epilogue warps
-  static constexpr int kStagingBytes = 8 * 4096;        // 8 epilogue warps x (32 rows x 128 B) / 16 x (32 rows x 64 B)
+  static constexpr int kAccBytes = BM * BN * 4;           // the fp32 accumulator tile handed to the epilogue
+  static constexpr int kStagingBytes = 8 * 4096;          // 8 epilogue warps x (32 rows x 128 B)
   static constexpr int kBiasBytes = BN * 4;
-  static constexpr int kRope = EPI == 2 ? kRopeBytes : 0;   // (EPI 3 reuses s_bias only)
-  static constexpr int kSmem = kStages * kStageBytes + kStagingBytes + kBiasBytes + kRope + 1024 /*align*/ + 256 /*barriers*/;
-  static constexpr int kHaloStages = BN <= 32 ? 6 : 5;
-  static constexpr int kSmemHalo = kHaloStages * kHaloStageBytes + 9 * kBBytes + kStagingBytes + kBiasBytes + 1024 + 256;
-  static constexpr int kTmemCols = 2 * BN < 32 ? 32 : 2 * BN;
+  static constexpr int kRope = EPI == 2 ? kRopeBytes : 0;
+  static constexpr int kFixed = kAccBytes + kStagingBytes + kBiasBytes + kRope + 1024 /*align*/ + 256 /*barriers*/;
+  static constexpr int kStages = (kSmemMax - kFixed) / kStageBytes > 8 ? 8 : (kSmemMax - kFixed) / kStageBytes;
+  static constexpr int kSmem = kStages * kStageBytes + kFixed;
+  static constexpr int kConsumerWarps = 8;
+  static constexpr int kThreads = 32 * kConsumerWarps + 32;   // two consumer warpgroups + the producer warp
+  static_assert(kStages >= 3, "shared-memory budget");
 };
+
+// byte offset of accumulator (row, col) in the fp32 tile: 16-byte chunk c of a row sits at chunk c ^ (row & 7) of its
+// 128-byte group, so that both the fragment stores and the row-per-thread loads of 8 consecutive rows spread over all banks
+template <int BN>
+__device__ __forceinline__ uint32_t acc_off(int row, int col) {
+  return static_cast<uint32_t>(row * (BN * 4) + ((((col >> 2) ^ (row & 7))) << 4) + ((col & 3) << 2));
+}
+// 32 consecutive accumulator columns of one tile row
+template <int BN>
+__device__ __forceinline__ void acc_ld32_t(uint32_t base, int row, int col, uint32_t (&v)[32]) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const uint32_t a = base + acc_off<BN>(row, col + 4 * i);
+    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v[4 * i]), "=r"(v[4 * i + 1]), "=r"(v[4 * i + 2]), "=r"(v[4 * i + 3]) : "r"(a) : "memory");
+  }
+}
+#define acc_ld32(base, row, col, v) acc_ld32_t<BN>(base, row, col, v)
 
 template <int kEpiThreads = 256>
 __device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kEpiThreads) : "memory"); }
@@ -99,7 +99,7 @@ __device__ __forceinline__ float gelu_fast(float x) {
   return fmaf(h, copysignf(er, x), h);
 }
 
-// the same for two values in packed f32x2 instructions (7 FFMA2/FMUL2 + 4 MUFU + 4 sign ops per PAIR instead of 13 + 2 per value)
+// the same for the two values of a float2
 __device__ __forceinline__ float2 gelu_fast2(float2 x) {
   const float2 ax = make_float2(fabsf(x.x), fabsf(x.y));
   const float2 u = fma2(make_float2(0.3275911f * 0.70710678118654752440f, 0.3275911f * 0.70710678118654752440f), ax, make_float2(1.0f, 1.0f));
@@ -139,54 +139,32 @@ __device__ __forceinline__ void act_vec(float (&f)[NV]) {
   }
 }
 
-// EPI: 0 = generic 16-bit out, 1 = generic fp32 out, 2 = QKV(+RoPE, head split), 3 = SwiGLU (silu(x1)*x2), 4 = lean 16-bit out
-// (bias -> 16-bit rounding -> ACT1 only, 16 epilogue warps; CTA pairs).  ACT1 / ACT2: compile-time activations
-// after the bias / after the affine (B2U_ACT_*), so the fully unrolled epilogue stays small enough for the I-cache.
-template <int BN, int EPI, int ACT1, int ACT2, typename T, bool PAIR = false>
-__global__ void __launch_bounds__((Cfg2<BN, EPI, PAIR>::kThreads), 1) gemm_tc2_kernel(const __grid_constant__ GemmMaps maps, const GemmArgs args) {
-  using C = Cfg2<BN, EPI, PAIR>;
+// EPI: 0 = generic 16-bit out, 1 = generic fp32 out, 2 = QKV(+RoPE, head split), 3 = SwiGLU (silu(x1)*x2).  ACT1 / ACT2:
+// compile-time activations after the bias / after the affine (B2U_ACT_*), so the fully unrolled epilogue stays small enough
+// for the I-cache.
+template <int BN, int EPI, int ACT1, int ACT2, typename T>
+__global__ void __launch_bounds__((Cfg2<BN, EPI>::kThreads), 1) gemm_tc2_kernel(const __grid_constant__ GemmMaps maps, const GemmArgs args) {
+  using C = Cfg2<BN, EPI>;
   using TT = T16<T>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  // conv == 3 ("halo" mode): stages hold one [3 rows][130 px][128 B] input halo each, followed by the 9 resident weight
-  // taps; otherwise the {A, W} k-block ring of Cfg2.  (Barrier arrays are sized for the larger stage count.)
-  const bool halo = args.conv == 3;
-  const int nstages = halo ? args.halo_stages : C::kStages;
-  const int stage_bytes = halo ? kHaloStageBytes : C::kStageBytes;
-  uint8_t* s_wtaps = smem + nstages * stage_bytes;                       // halo mode only: 9 x [BN x 128 B]
-  uint8_t* staging = s_wtaps + (halo ? 9 * C::kBBytes : 0);
+  uint8_t* s_acc = smem + C::kStages * C::kStageBytes;
+  uint8_t* staging = s_acc + C::kAccBytes;
   float* s_bias = reinterpret_cast<float*>(staging + C::kStagingBytes);
   float* s_rope = reinterpret_cast<float*>(staging + C::kStagingBytes + C::kBiasBytes);   // [h+w][2*hq + 4] = (sin | cos | pad)
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + C::kStagingBytes + C::kBiasBytes + C::kRope);
   uint64_t* empty_bar = full_bar + 8;
-  uint64_t* tfull_bar = empty_bar + 8;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint64_t* w_bar = tempty_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(w_bar + 1);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  // PAIR: the cluster (CTA pair) is the scheduling unit; tile = (pair of m-tiles, n-tile); this CTA owns m-tile 2*mp + rank
-  const uint32_t cta_rank = PAIR ? cluster_ctarank() : 0u;
-  const int unit_id = PAIR ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-  const int unit_cnt = PAIR ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
-  const long long total_tiles = PAIR ? static_cast<long long>((args.m_tiles + 1) / 2) * args.n_tiles
-                                     : static_cast<long long>(args.m_tiles) * args.n_tiles;
+  const long long total_tiles = static_cast<long long>(args.m_tiles) * args.n_tiles;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&maps.a[0]);
     tma_prefetch_desc(&maps.b);
-    for (int s = 0; s < 8; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(w_bar, 1);
-    // BN <= 32: a tile is one 32-column chunk, drained by ONE warp per TMEM lane quarter; the two warp sets alternate
-    // tiles (set = accumulator buffer), so two epilogues are in flight instead of one set idling
-    for (int s = 0; s < 2; ++s) { mbar_init(&tfull_bar[s], 1); mbar_init(&tempty_bar[s], PAIR ? 2 * C::kEpiWarps : (BN <= 32 ? 4 : C::kEpiWarps)); }
+    // a stage is free again once every consumer warp has seen the MMAs that read it complete
+    for (int s = 0; s < 8; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], C::kConsumerWarps); }
     fence_mbar_init();
-  }
-  if constexpr (PAIR) cluster_sync_all();   // the peer's barriers exist before any remote arrive / multicast commit
-  if (warp == 1) {
-    if constexpr (PAIR) { tmem_alloc2(tmem_slot, C::kTmemCols); tmem_relinquish2(); }
-    else { tmem_alloc(tmem_slot, C::kTmemCols); tmem_relinquish(); }
   }
   if constexpr (EPI == 2) {
     if (args.rope_w > 0) {
@@ -204,38 +182,17 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI, PAIR>::kThreads), 1) gemm_tc2_k
       }
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();                              // barriers, TMEM and tensor maps are set up: now wait for the producer kernel's data
+  pdl_wait();                              // barriers and tensor maps are set up: now wait for the producer kernel's data
 
-  if (warp == 0) {
+  if (warp == C::kConsumerWarps) {
     // ===================== TMA producer =====================
     if (elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
-      if (halo) {   // the 9 weight taps stay resident in smem for the whole kernel (n_tiles == 1)
-        mbar_expect_tx(w_bar, 9 * C::kBBytes);
-        for (int tap = 0; tap < 9; ++tap) tma_load_2d(s_wtaps + tap * C::kBBytes, &maps.b, w_bar, tap * BK, 0);
-      }
-      const uint32_t full0 = PAIR ? mapa_u32(smem_u32(full_bar), 0) : 0u;   // the leader CTA's full barriers
-      for (long long tile = unit_id; tile < total_tiles; tile += unit_cnt) {
+      for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const int nt = static_cast<int>(tile % args.n_tiles);
-        const int mt = PAIR ? 2 * static_cast<int>(tile / args.n_tiles) + static_cast<int>(cta_rank)
-                            : static_cast<int>(tile / args.n_tiles);
-        if constexpr (PAIR) {
-          // both CTAs post their bytes on the LEADER's full barrier; only the leader arms it (for both halves)
-          for (int kb = 0; kb < args.num_kb; ++kb) {
-            mbar_wait(&empty_bar[stage], phase ^ 1);
-            uint8_t* sA = smem + stage * C::kStageBytes;
-            if (cta_rank == 0) mbar_expect_tx(&full_bar[stage], 2 * C::kStageBytes);
-            tma_load_2d_pair(sA, &maps.a[0], full0 + stage * 8, kb * BK, mt * BM);
-            tma_load_2d_pair(sA + C::kABytes, &maps.b, full0 + stage * 8, kb * BK, nt * BN + static_cast<int>(cta_rank) * (BN / 2));
-            if (++stage == C::kStages) { stage = 0; phase ^= 1; }
-          }
-          continue;
-        }
+        const int mt = static_cast<int>(tile / args.n_tiles);
         int img = 0, y0 = 0, x0 = 0;
         if (args.conv) {
           const int per_img = args.tiles_x * args.tiles_y;
@@ -243,26 +200,6 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI, PAIR>::kThreads), 1) gemm_tc2_k
           const int r = mt - img * per_img;
           y0 = (r / args.tiles_x) * args.TH;
           x0 = (r % args.tiles_x) * args.TW;
-        }
-        if (halo) {
-          // The ring holds only 2-3 of these 49 KB boxes, so the tile rate is (stages / load latency): pull the box this CTA
-          // will need kHaloPrefetch tiles from now into L2, so that its TMA load later costs an L2 hit, not a DRAM miss.
-          {
-            const long long tf = tile + static_cast<long long>(kHaloPrefetch) * unit_cnt;
-            if (tf < total_tiles) {
-              const int mtf = static_cast<int>(tf / args.n_tiles);
-              const int per_img = args.tiles_x * args.tiles_y;
-              const int imgf = mtf / per_img;
-              const int rf = mtf - imgf * per_img;
-              tma_prefetch_4d(&maps.a[0], 0, (rf % args.tiles_x) * args.TW - 1, (rf / args.tiles_x) * args.TH - 1, imgf);
-            }
-          }
-          // one TMA box per tile: channels [0,64) x pixels [x0-1, x0+9) x rows [y0-1, y0+17) (OOB = zero padding)
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          mbar_expect_tx(&full_bar[stage], kHaloBytes);
-          tma_load_4d(smem + stage * stage_bytes, &maps.a[0], &full_bar[stage], 0, x0 - 1, y0 - 1, img);
-          if (++stage == nstages) { stage = 0; phase ^= 1; }
-          continue;
         }
         for (int kb = 0; kb < args.num_kb; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
@@ -288,91 +225,56 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI, PAIR>::kThreads), 1) gemm_tc2_k
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (cta_rank == 0 && elect_one()) {
-      constexpr uint32_t idesc = make_idesc_f16(TT::kFmt, PAIR ? 2 * BM : BM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (long long tile = unit_id; tile < total_tiles; tile += unit_cnt, ++it) {
-        const int buf = it & 1;
-        mbar_wait(&tempty_bar[buf], ((it >> 1) & 1) ^ 1);   // epilogue has drained this accumulator buffer
-        tc_fence_after();
-        const uint32_t tacc = tmem_base + buf * BN;
-        if constexpr (PAIR) {
-          for (int kb = 0; kb < args.num_kb; ++kb) {
-            mbar_wait(&full_bar[stage], phase);
-            tc_fence_after();
-            const uint32_t sA = smem_u32(smem + stage * C::kStageBytes);
-            const uint64_t da = make_desc_k128(sA);
-            const uint64_t db = make_desc_k128(sA + C::kABytes);
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k)
-              tc_mma_f16_pair(tacc, da + static_cast<uint64_t>(k * 2), db + static_cast<uint64_t>(k * 2), idesc, (kb | k) != 0 ? 1u : 0u);
-            tc_commit_pair(&empty_bar[stage], 3);      // frees the stage in BOTH CTAs
-            if (++stage == C::kStages) { stage = 0; phase ^= 1; }
-          }
-          tc_commit_pair(&tfull_bar[buf], 3);          // both CTAs' epilogues drain their 128 rows
-          continue;
-        }
-        if (halo) {
-          if (it == 0) { mbar_wait(w_bar, 0); }
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sH = smem_u32(smem + stage * stage_bytes);
-          const uint32_t sW = smem_u32(s_wtaps);
-#pragma unroll
-          for (int tap = 0; tap < 9; ++tap) {       // fully unrolled: every descriptor is base + compile-time constant
-            const int dy = tap / 3, dx = tap - dy * 3;
-            // A = the 16 x 8 pixel window of the halo tile that starts at halo pixel (dy, dx): 8-pixel groups, one per halo row.
-            // Its start is only 128 B-aligned; measured on B200 (tools/halo_probe.py): the 128B swizzle is a function of the
-            // absolute smem address, so the descriptor needs NO base_offset (setting it to (addr>>7)&7 gives wrong data).
-            const uint32_t aaddr = sH + (dy * kHaloW + dx) * 128;
-            const uint64_t da = make_desc_k128_sbo(aaddr, kHaloW * 128);
-            const uint64_t db = make_desc_k128(sW + tap * C::kBBytes);
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k)
-              tc_mma_f16(tacc, da + static_cast<uint64_t>(k * 2), db + static_cast<uint64_t>(k * 2), idesc, (tap | k) != 0 ? 1u : 0u);
-          }
-          tc_commit(&empty_bar[stage]);
-          if (++stage == nstages) { stage = 0; phase ^= 1; }
-        } else {
-        for (int kb = 0; kb < args.num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sA = smem_u32(smem + stage * C::kStageBytes);
-          const uint64_t da = make_desc_k128(sA);
-          const uint64_t db = make_desc_k128(sA + C::kABytes);
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k)
-            tc_mma_f16(tacc, da + static_cast<uint64_t>(k * 2), db + static_cast<uint64_t>(k * 2), idesc, (kb | k) != 0 ? 1u : 0u);
-          tc_commit(&empty_bar[stage]);
-          if (++stage == C::kStages) { stage = 0; phase ^= 1; }
-        }
-        }
-        tc_commit(&tfull_bar[buf]);
-      }
-    }
   } else {
-    // ===================== epilogue warps (2..9; EPI 4: 2..17) =====================
-    const int q4 = warp & 3;
-    const int ew = warp - 2;                         // staging patch index
-    const int half = ew >> 2;                        // which half of the tile's columns this warp drains
+    // ===================== consumer warpgroups: MMA, then the epilogue =====================
+    const int wg = warp >> 2;                        // tile rows [64 wg, 64 wg + 64) of the MMA
+    const int q4 = warp & 3;                         // epilogue: tile rows [32 q4, 32 q4 + 32), one per lane
+    const int ew = warp;                             // staging patch index
+    const int half = warp >> 2;                      // which half of the tile's columns this warp drains
+    const int arow = q4 * 32 + lane;
     uint8_t* patch = staging + ew * 4096;
     const uint32_t patch_u32 = smem_u32(patch);
+    const uint32_t acc_u32 = smem_u32(s_acc);
     const b2u_epilogue& e = args.epi;
-    const int etid = threadIdx.x - 64;               // 0..127 among epilogue threads
-    int it = 0;
-    const uint32_t tempty0 = PAIR ? mapa_u32(smem_u32(tempty_bar), 0) : 0u;   // the leader CTA's "accumulator drained" barriers
-    for (long long tile = unit_id; tile < total_tiles; tile += unit_cnt, ++it) {
-      const int buf = it & 1;
-      if constexpr (BN <= 32) {
-        if (buf != half) continue;                     // the other warp set owns this accumulator buffer
-      }
+    const int etid = threadIdx.x;                    // 0..255 among epilogue threads
+    int stage = 0;
+    uint32_t phase = 0;
+    for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int nt = static_cast<int>(tile % args.n_tiles);
-      const int mt = PAIR ? 2 * static_cast<int>(tile / args.n_tiles) + static_cast<int>(cta_rank)
-                          : static_cast<int>(tile / args.n_tiles);
+      const int mt = static_cast<int>(tile / args.n_tiles);
+      float acc[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < args.num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sA = smem_u32(smem + stage * C::kStageBytes);
+        const uint64_t da = make_gdesc_k128(sA + wg * 64 * 128);
+        const uint64_t db = make_gdesc_k128(sA + C::kABytes);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k)
+          wgmma_ss<TT::kFmt, BN>(acc, da + static_cast<uint64_t>(k * 2), db + static_cast<uint64_t>(k * 2), (kb | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();                             // the previous k-block's MMAs are done: its stage may be refilled
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == C::kStages) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      // accumulator fragments -> s_acc (row-major fp32)
+      epi_bar_sync();                                // the previous tile's epilogue has finished reading s_acc
+      {
+        const int r0 = wg * 64 + q4 * 16 + (lane >> 2);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int c = 8 * j + 2 * (lane & 3);
+          asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(acc_u32 + acc_off<BN>(r0, c)), "f"(acc[4 * j]), "f"(acc[4 * j + 1]) : "memory");
+          asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(acc_u32 + acc_off<BN>(r0 + 8, c)), "f"(acc[4 * j + 2]), "f"(acc[4 * j + 3]) : "memory");
+        }
+      }
+      epi_bar_sync();
       const int n0 = nt * BN;
       int img = 0, y0 = 0, x0 = 0;
       if (args.conv) {
@@ -394,139 +296,8 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI, PAIR>::kThreads), 1) gemm_tc2_k
         return (y < args.Ho) && (x < args.Wo);
       };
 
-      if constexpr (EPI == 2 && C::kEpiWarps == 16) {
-        // ---- QKV epilogue on sixteen warps (four per TMEM lane quarter): warp = one 64-column unit (32 low + 32 matching
-        // high rope columns of a head), drained as two passes of 16 + 16 columns so that it fits 96 registers and a 64 B
-        // staging row.  No barrier among the warps (bias through L1 as warp-uniform loads).
-        const int HDm = args.head_dim;                 // 64 or 128
-        const int hq = HDm >> 2;                       // angles per axis (rope_position_encoding.py: D_head / 4)
-        long long m1;
-        const bool v1 = row_of(q4 * 32 + lane, m1);   // phase-1 owner row
-        const unsigned ntok_u = static_cast<unsigned>(args.ntok);   // token rows fit 32 bits (host-checked): 32-bit divides
-        const int b1 = static_cast<int>(static_cast<unsigned>(m1) / ntok_u);
-        const int t1 = static_cast<int>(static_cast<unsigned>(m1) - static_cast<unsigned>(b1) * ntok_u);
-        const bool rot = v1 && t1 >= args.prefix;
-        long long dst_off[4];                          // phase-2 rows of this lane: rr = i*8 + lane/4 (4 lanes x 16 B per row)
-        bool dst_ok[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          long long m2;
-          dst_ok[i] = row_of(q4 * 32 + i * 8 + (lane >> 2), m2);
-          const int b2 = static_cast<int>(static_cast<unsigned>(m2) / ntok_u);
-          const int t2 = static_cast<int>(static_cast<unsigned>(m2) - static_cast<unsigned>(b2) * ntok_u);
-          dst_off[i] = (static_cast<long long>(b2) * args.heads * args.ntok + t2) * HDm;
-        }
-        const uint32_t patch4_u32 = smem_u32(staging + ew * 2048);
-        const int u = half;                            // = ew >> 2 in 0..3: the unit of this warp
-        const int hcol = HDm == 64 ? u * 64 : (u >> 1) * 128;          // first accumulator column of the head
-        const int pss = HDm == 64 ? 0 : (u & 1);
-        const int n = n0 + hcol;
-        const bool live = n < args.N;                  // warp-uniform
-        const int which = n / args.D;
-        const int head = (n - which * args.D) / HDm;
-        mbar_wait(&tfull_bar[buf], (it >> 1) & 1);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + buf * BN + (static_cast<uint32_t>(q4 * 32) << 16);
-#pragma unroll 1
-        for (int ps = 0; ps < 2; ++ps) {
-          const int lo_off = pss * 32 + ps * 16, hi_off = (HDm >> 1) + pss * 32 + ps * 16;    // element offsets inside the head
-          uint32_t v0[16], v1r[16];
-          tmem_ld16(taddr + hcol + lo_off, v0);
-          tmem_ld16(taddr + hcol + hi_off, v1r);
-          tmem_ld_wait();
-          if (ps == 1) {                               // the accumulator is in registers: hand the buffer back before the math
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-              if constexpr (PAIR) mbar_arrive_cluster(tempty0 + buf * 8);
-              else mbar_arrive(&tempty_bar[buf]);
-            }
-          }
-          if (!live) continue;
-          float x[32];
-#pragma unroll
-          for (int j = 0; j < 16; j += 4) {   // Linear output rounded to 16 bits (packed add: FADD2; packed converts: F2FP)
-            const float4 blo = e.bias ? __ldg(reinterpret_cast<const float4*>(e.bias + n + lo_off + j)) : make_float4(0.f, 0.f, 0.f, 0.f);
-            const float4 bhi = e.bias ? __ldg(reinterpret_cast<const float4*>(e.bias + n + hi_off + j)) : make_float4(0.f, 0.f, 0.f, 0.f);
-            const float2 l01 = round16v<TT>((add2(make_float2(__uint_as_float(v0[j]), __uint_as_float(v0[j + 1])), make_float2(blo.x, blo.y))));
-            const float2 l23 = round16v<TT>((add2(make_float2(__uint_as_float(v0[j + 2]), __uint_as_float(v0[j + 3])), make_float2(blo.z, blo.w))));
-            const float2 h01 = round16v<TT>((add2(make_float2(__uint_as_float(v1r[j]), __uint_as_float(v1r[j + 1])), make_float2(bhi.x, bhi.y))));
-            const float2 h23 = round16v<TT>((add2(make_float2(__uint_as_float(v1r[j + 2]), __uint_as_float(v1r[j + 3])), make_float2(bhi.z, bhi.w))));
-            x[j] = l01.x; x[j + 1] = l01.y; x[j + 2] = l23.x; x[j + 3] = l23.y;
-            x[16 + j] = h01.x; x[17 + j] = h01.y; x[18 + j] = h23.x; x[19 + j] = h23.y;
-          }
-          if (which == 2 && args.npad > 0) {
-            // V^T [B, heads, head_dim, npad]: lane = token, loop over d -> each store instruction writes 32 consecutive keys
-            if (v1) {
-              T* dst = reinterpret_cast<T*>(args.v) + (static_cast<long long>(b1) * args.heads + head) * HDm * args.npad + t1;
-#pragma unroll
-              for (int j = 0; j < 16; ++j) {
-                dst[static_cast<long long>(lo_off + j) * args.npad] = TT::from_f(x[j]);
-                dst[static_cast<long long>(hi_off + j) * args.npad] = TT::from_f(x[16 + j]);
-              }
-            }
-            continue;   // warp-uniform
-          }
-          uint32_t packed[16];
-          if (which < 2 && rot && args.rope_w > 0) {
-            // separable tables from smem ([h + w] rows of (sin[hq] | cos[hq] | pad)): angle A < hq comes from the patch row's
-            // table, A >= hq from the patch column's; cos/sin[A + head_dim/2] == cos/sin[A]
-            const int pidx = t1 - args.prefix;
-            const int py = pidx / args.rope_w, px = pidx - py * args.rope_w;
-            const uint32_t rstride = hq * 8 + 16;      // padded rows: the 32 lanes' column-table rows hit distinct banks
-            const uint32_t ry = smem_u32(s_rope) + py * rstride, rx = smem_u32(s_rope) + (args.rope_h + px) * rstride;
-#pragma unroll
-            for (int j = 0; j < 16; j += 4) {
-              const int A = lo_off + j;                // angle index in [0, head_dim/2)
-              const uint32_t rbase_ = (A < hq ? ry : rx) + (A & (hq - 1)) * 4;
-              const float4 sn = lds128f(rbase_), cs = lds128f(rbase_ + hq * 4);
-              // rotation in packed f32x2: lo' = lo*cos - hi*sin, hi' = hi*cos + lo*sin (two angles per instruction)
-              const float2 c01 = make_float2(cs.x, cs.y), c23 = make_float2(cs.z, cs.w);
-              const float2 s01 = make_float2(sn.x, sn.y), s23 = make_float2(sn.z, sn.w);
-              const float2 l01 = make_float2(x[j], x[j + 1]), l23 = make_float2(x[j + 2], x[j + 3]);
-              const float2 h01 = make_float2(x[j + 16], x[j + 17]), h23 = make_float2(x[j + 18], x[j + 19]);
-              const float2 a01 = fma2(l01, c01, mul2(h01, make_float2(-s01.x, -s01.y)));
-              const float2 a23 = fma2(l23, c23, mul2(h23, make_float2(-s23.x, -s23.y)));
-              const float2 b01 = fma2(h01, c01, mul2(l01, s01));
-              const float2 b23 = fma2(h23, c23, mul2(l23, s23));
-              packed[j / 2] = TT::pack2(a01.x, a01.y);
-              packed[j / 2 + 1] = TT::pack2(a23.x, a23.y);
-              packed[8 + j / 2] = TT::pack2(b01.x, b01.y);
-              packed[8 + j / 2 + 1] = TT::pack2(b23.x, b23.y);
-            }
-          } else if (which < 2 && rot) {
-            const float* sinr = args.rope_sin + static_cast<long long>(t1 - args.prefix) * HDm;
-            const float* cosr = args.rope_cos + static_cast<long long>(t1 - args.prefix) * HDm;
-#pragma unroll
-            for (int j = 0; j < 16; j += 4) {
-              const float4 c_lo = *reinterpret_cast<const float4*>(cosr + lo_off + j), s_lo = *reinterpret_cast<const float4*>(sinr + lo_off + j);
-              const float4 c_hi = *reinterpret_cast<const float4*>(cosr + hi_off + j), s_hi = *reinterpret_cast<const float4*>(sinr + hi_off + j);
-              packed[j / 2] = TT::pack2(x[j] * c_lo.x - x[j + 16] * s_lo.x, x[j + 1] * c_lo.y - x[j + 17] * s_lo.y);
-              packed[j / 2 + 1] = TT::pack2(x[j + 2] * c_lo.z - x[j + 18] * s_lo.z, x[j + 3] * c_lo.w - x[j + 19] * s_lo.w);
-              packed[8 + j / 2] = TT::pack2(x[j + 16] * c_hi.x + x[j] * s_hi.x, x[j + 17] * c_hi.y + x[j + 1] * s_hi.y);
-              packed[8 + j / 2 + 1] = TT::pack2(x[j + 18] * c_hi.z + x[j + 2] * s_hi.z, x[j + 19] * c_hi.w + x[j + 3] * s_hi.w);
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; j += 2) packed[j / 2] = TT::pack2(x[j], x[j + 1]);
-          }
-          // stage: row = lane, 4 x 16 B chunks (2 of the lo segment, 2 of the hi segment), chunk position c ^ ((row >> 1) & 3)
-          __syncwarp();
-#pragma unroll
-          for (int c = 0; c < 4; ++c)
-            sts128(patch4_u32 + lane * 64 + ((c ^ ((lane >> 1) & 3)) << 4), packed[4 * c], packed[4 * c + 1], packed[4 * c + 2], packed[4 * c + 3]);
-          __syncwarp();
-          T* base = reinterpret_cast<T*>(which == 0 ? args.q : (which == 1 ? args.k : args.v)) +
-                    static_cast<long long>(head) * args.ntok * HDm + ((lane & 2) ? hi_off : lo_off) + (lane & 1) * 8;
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int rr = i * 8 + (lane >> 2);
-            const uint4 val = lds128(patch4_u32 + rr * 64 + (((lane & 3) ^ ((rr >> 1) & 3)) << 4));
-            if (dst_ok[i]) *reinterpret_cast<uint4*>(base + dst_off[i]) = val;
-          }
-        }
-        continue;   // the accumulator buffer was released above
-      } else if constexpr (EPI == 2) {
+
+      if constexpr (EPI == 2) {
         // stage the (masked) bias of this tile's columns once
         epi_bar_sync();
         for (int i = etid; i < BN; i += 256) s_bias[i] = (e.bias && n0 + i < args.N) ? __ldg(e.bias + n0 + i) : 0.f;
@@ -553,9 +324,6 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI, PAIR>::kThreads), 1) gemm_tc2_k
           const int t2 = static_cast<int>(static_cast<unsigned>(m2) - static_cast<unsigned>(b2) * ntok_u);
           dst_off[i] = (static_cast<long long>(b2) * args.heads * args.ntok + t2) * HDm;
         }
-        mbar_wait(&tfull_bar[buf], (it >> 1) & 1);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + buf * BN + (static_cast<uint32_t>(q4 * 32) << 16);
         // A "unit" = 64 accumulator columns = the 32 low + 32 matching high rope columns of one head:
         //   head_dim 64 : unit u = head u of the tile, lo = [0,32), hi = [32,64)
         //   head_dim 128: unit u = (head u/2, pass p = u&1), lo = [32p, 32p+32), hi = [64+32p, 64+32p+32)
@@ -565,16 +333,15 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI, PAIR>::kThreads), 1) gemm_tc2_k
           const int pss = HDm == 64 ? 0 : (u & 1);
           const int lo_off = pss * 32, hi_off = (HDm >> 1) + pss * 32;    // element offsets inside the head
           uint32_t v0[32], v1r[32];
-          tmem_ld32(taddr + hcol + lo_off, v0);
-          tmem_ld32(taddr + hcol + hi_off, v1r);
-          tmem_ld_wait();
+          acc_ld32(acc_u32, arow, hcol + lo_off, v0);
+          acc_ld32(acc_u32, arow, hcol + hi_off, v1r);
           const int n = n0 + hcol;
           if (n >= args.N) continue;   // warp-uniform
           const int which = n / args.D;
           const int head = (n - which * args.D) / HDm;
           float x[64];
 #pragma unroll
-          for (int j = 0; j < 32; j += 2) {   // Linear output rounded to 16 bits (packed add: FADD2; packed converts: F2FP)
+          for (int j = 0; j < 32; j += 2) {   // Linear output rounded to 16 bits
             const float2 blo = *reinterpret_cast<const float2*>(&s_bias[hcol + lo_off + j]);
             const float2 bhi = *reinterpret_cast<const float2*>(&s_bias[hcol + hi_off + j]);
             const float2 alo = add2(make_float2(__uint_as_float(v0[j]), __uint_as_float(v0[j + 1])), blo);
@@ -611,7 +378,7 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI, PAIR>::kThreads), 1) gemm_tc2_k
               const int A = lo_off + j;                // angle index in [0, head_dim/2)
               const uint32_t rbase_ = (A < hq ? ry : rx) + (A & (hq - 1)) * 4;
               const float4 sn = lds128f(rbase_), cs = lds128f(rbase_ + hq * 4);
-              // rotation in packed f32x2: lo' = lo*cos - hi*sin, hi' = hi*cos + lo*sin (two angles per instruction)
+              // rotation: lo' = lo*cos - hi*sin, hi' = hi*cos + lo*sin (two angles per instruction)
               const float2 c01 = make_float2(cs.x, cs.y), c23 = make_float2(cs.z, cs.w);
               const float2 s01 = make_float2(sn.x, sn.y), s23 = make_float2(sn.z, sn.w);
               const float2 l01 = make_float2(x[j], x[j + 1]), l23 = make_float2(x[j + 2], x[j + 3]);
@@ -669,15 +436,11 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI, PAIR>::kThreads), 1) gemm_tc2_k
           dst_ok[i] = row_of(q4 * 32 + i * 8 + (lane >> 2), m2);
           dst_row[i] = dst_ok[i] ? m2 : 0;
         }
-        mbar_wait(&tfull_bar[buf], (it >> 1) & 1);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + buf * BN + (static_cast<uint32_t>(q4 * 32) << 16);
 #pragma unroll 1
         for (int g = half * (BN / 128); g < (half + 1) * (BN / 128); ++g) {
           uint32_t v0[32], v1r[32];
-          tmem_ld32(taddr + g * 64, v0);
-          tmem_ld32(taddr + g * 64 + 32, v1r);
-          tmem_ld_wait();
+          acc_ld32(acc_u32, arow, g * 64, v0);
+          acc_ld32(acc_u32, arow, g * 64 + 32, v1r);
           const int n = n0 + g * 64;
           if (n >= args.N) continue;   // warp-uniform
           uint32_t packed[16];
@@ -707,86 +470,18 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI, PAIR>::kThreads), 1) gemm_tc2_k
             if (dst_ok[i]) *reinterpret_cast<uint4*>(reinterpret_cast<T*>(e.out) + dst_row[i] * e.ldc + ocol) = val;
           }
         }
-      } else if constexpr (EPI == 4) {
-        // ---- lean 16-bit epilogue (ViT fc1: bias -> Linear output rounded to 16 bits -> GELU).  Measured with ncu on the
-        // generic path: the MMA never waits for operands but for an accumulator buffer - eight epilogue warps (two per
-        // scheduler) run the dependent GELU chains at 0.2 IPC.  Here SIXTEEN warps drain a tile (four per TMEM lane
-        // quarter, two 32-column chunks each), the math runs on the TMEM registers (thread = accumulator row) and only the
-        // packed 16-bit result goes through the staging transpose.  (Standalone at the fc1 shape: 242 -> 213 us.)
-        // (no barrier among the epilogue warps: the bias comes through L1 as warp-uniform loads, each warp runs on its own)
-        long long dst_row[4];
-        bool dst_ok[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {             // phase-2 rows: rr = i*8 + lane/4 (4 lanes x 16 B = one 64 B row segment)
-          long long m2;
-          dst_ok[i] = row_of(q4 * 32 + i * 8 + (lane >> 2), m2);
-          dst_row[i] = dst_ok[i] ? m2 : 0;
-        }
-        uint8_t* patch4 = staging + ew * 2048;
-        const uint32_t patch4_u32 = smem_u32(patch4);
-        mbar_wait(&tfull_bar[buf], (it >> 1) & 1);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + buf * BN + (static_cast<uint32_t>(q4 * 32) << 16);
-        constexpr int kPerWarp = BN / 32 / 4;            // chunks per warp (2 for BN 256)
-#pragma unroll 1
-        for (int cc = 0; cc < kPerWarp; ++cc) {
-          const int ch = half * kPerWarp + cc;           // half = ew >> 2 in 0..3 here
-          uint32_t v[32];
-          tmem_ld32(taddr + ch * 32, v);
-          tmem_ld_wait();
-          if (cc == kPerWarp - 1) {                      // the accumulator is in registers: hand the buffer back before the math
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-              if constexpr (PAIR) mbar_arrive_cluster(tempty0 + buf * 8);
-              else mbar_arrive(&tempty_bar[buf]);
-            }
-          }
-          const int n = n0 + ch * 32;
-          if (n >= args.N) continue;   // warp-uniform
-          uint32_t packed[16];
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 b4 = e.bias ? __ldg(reinterpret_cast<const float4*>(e.bias + n + j)) : make_float4(0.f, 0.f, 0.f, 0.f);
-            float2 a01 = add2(make_float2(__uint_as_float(v[j]), __uint_as_float(v[j + 1])), make_float2(b4.x, b4.y));
-            float2 a23 = add2(make_float2(__uint_as_float(v[j + 2]), __uint_as_float(v[j + 3])), make_float2(b4.z, b4.w));
-            if (e.round16) {
-              a01 = TT::unpack2(TT::pack2(a01.x, a01.y));
-              a23 = TT::unpack2(TT::pack2(a23.x, a23.y));
-            }
-            float f[4] = {a01.x, a01.y, a23.x, a23.y};
-            act_vec<ACT1, 4>(f);
-            packed[j / 2] = TT::pack2(f[0], f[1]);
-            packed[j / 2 + 1] = TT::pack2(f[2], f[3]);
-          }
-          // stage: row = lane, 64 B of output (4 x 16 B chunks) at chunk position c ^ ((row >> 1) & 3) within a 64 B slot
-          __syncwarp();
-#pragma unroll
-          for (int c = 0; c < 4; ++c)
-            sts128(patch4_u32 + lane * 64 + ((c ^ ((lane >> 1) & 3)) << 4), packed[4 * c], packed[4 * c + 1], packed[4 * c + 2], packed[4 * c + 3]);
-          __syncwarp();
-          const int ocol = n + (lane & 3) * 8 + e.col_off;
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int rr = i * 8 + (lane >> 2);
-            const uint4 val = lds128(patch4_u32 + rr * 64 + (((lane & 3) ^ ((rr >> 1) & 3)) << 4));
-            if (dst_ok[i]) *reinterpret_cast<uint4*>(reinterpret_cast<T*>(e.out) + dst_row[i] * e.ldc + ocol) = val;
-          }
-        }
-        continue;   // the accumulator buffer was released above
       } else {
         // ---- phase-2 row assignment: fp32 output -> 8 lanes per row (4 cols each), 4 rows per pass, 8 passes;
         //                              16-bit output -> 4 lanes per row (8 cols each), 8 rows per pass, 4 passes.
         constexpr bool o32 = (EPI == 1);
         if constexpr (BN >= 64) {
-          // Short-K GEMMs with an fp32 residual stream (extractor out-proj / ffn2: 256 KB of residual read + write per tile
-          // against 2-3 us of MMA) are bound by the LATENCY of these residual loads - two warps per scheduler cannot keep
-          // enough bytes in flight.  Pull the NEXT tile's residual rows into L2 now, one tile ahead of their use.
+          // Short-K GEMMs with an fp32 residual stream (extractor out-proj / ffn2) are bound by the latency of these residual
+          // loads.  Pull the NEXT tile's residual rows into L2 now, one tile ahead of their use.
           if (args.res_prefetch && e.residual != nullptr && args.conv == 0 && e.ps_cout == 0) {
-            const long long nx = tile + unit_cnt;
+            const long long nx = tile + gridDim.x;
             if (nx < total_tiles) {
               const int ntn = static_cast<int>(nx % args.n_tiles);
-              const long long mtn = PAIR ? 2 * (nx / args.n_tiles) + cta_rank : nx / args.n_tiles;
+              const long long mtn = nx / args.n_tiles;
               const long long mn = mtn * BM + (etid >> 1);
               if (mn < args.M && (ntn + 1) * BN <= args.N) {
                 long long row = mn;
@@ -830,17 +525,14 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI, PAIR>::kThreads), 1) gemm_tc2_k
             }
           }
         }
-        mbar_wait(&tfull_bar[buf], (it >> 1) & 1);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + buf * BN + (static_cast<uint32_t>(q4 * 32) << 16);
         constexpr int kChunks = BN / 32;
         constexpr int kPerHalf = kChunks >= 2 ? kChunks / 2 : 1;
         const int ch_begin = kChunks >= 2 ? half * kPerHalf : 0;
-        const int ch_end = kChunks >= 2 ? ch_begin + kPerHalf : 1;   // BN 32: the owning warp set takes the only chunk
+        const int ch_end = kChunks >= 2 ? ch_begin + kPerHalf : (half == 0 ? 1 : 0);   // BN 32: the first warp set takes the only chunk
 #pragma unroll 1
         for (int ch = ch_begin; ch < ch_end; ++ch) {
           uint32_t v[32];
-          tmem_ld32(taddr + ch * 32, v);
+          acc_ld32(acc_u32, arow, ch * 32, v);
           const int n = n0 + ch * 32;
           const bool live = n < args.N;   // warp-uniform
           int ocol = n + lcol;
@@ -851,7 +543,7 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI, PAIR>::kThreads), 1) gemm_tc2_k
             radd = static_cast<long long>(qd >> 1) * (2 * e.ps_w) + (qd & 1);
           }
           ocol += e.col_off;
-          // ---- prefetch residual / skip operands for every pass of this chunk (latency overlaps the TMEM load)
+          // ---- prefetch residual / skip operands for every pass of this chunk
           float4 res[8];
           uint4 add[4];
           if (live && e.residual) {
@@ -879,7 +571,7 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI, PAIR>::kThreads), 1) gemm_tc2_k
               for (int i = 0; i < 4; ++i) add[i] = *reinterpret_cast<const uint4*>(reinterpret_cast<const T*>(e.add16) + (rbase[i] + radd) * e.ldadd + ocol);
             }
           }
-          // per-column parameters of this lane (constant over the rows): loaded before the TMEM wait
+          // per-column parameters of this lane (constant over the rows)
           constexpr int NV = o32 ? 4 : 8;
           const bool affine = e.scale != nullptr || e.shift != nullptr;   // warp-uniform
           float bi[NV], sc[NV], sh[NV];
@@ -893,7 +585,6 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI, PAIR>::kThreads), 1) gemm_tc2_k
               if (e.shift) { const float4 t = __ldg(reinterpret_cast<const float4*>(e.shift + n + lcol + 4 * h)); sh[4 * h] = t.x; sh[4 * h + 1] = t.y; sh[4 * h + 2] = t.z; sh[4 * h + 3] = t.w; }
             }
           }
-          tmem_ld_wait();
           if (!live) continue;
           // stage raw fp32 accumulators: row = lane, 8 x 16 B groups at position j ^ (row & 7)
           __syncwarp();
@@ -976,80 +667,28 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI, PAIR>::kThreads), 1) gemm_tc2_k
           }
         }
       }
-      // this warp is done reading accumulator buffer `buf`
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if constexpr (PAIR) mbar_arrive_cluster(tempty0 + buf * 8);
-        else mbar_arrive(&tempty_bar[buf]);
-      }
     }
   }
   pdl_launch_dependents();   // this CTA's tiles are done: once every CTA is here the next kernel may start its prologue
-  tc_fence_before();
-  __syncthreads();
-  if constexpr (PAIR) cluster_sync_all();   // nobody leaves while the peer can still touch its smem / barriers / TMEM
-  if (warp == 1) {
-    tc_fence_after();
-    if constexpr (PAIR) tmem_dealloc2(tmem_base, C::kTmemCols);
-    else tmem_dealloc(tmem_base, C::kTmemCols);
-  }
 }
+#undef acc_ld32
 
 // ------------------------------------------------------------------------------------------------ host side
 template <int BN, int EPI, int ACT1, int ACT2, typename T>
-static int launch_pair2(const GemmMaps& maps, const GemmArgs& args, cudaStream_t stream) {
-  auto kern = gemm_tc2_kernel<BN, EPI, ACT1, ACT2, T, true>;
-  static bool configured_dev[64] = {};
-  bool& configured = configured_dev[current_device_index()];
-  constexpr int kSmem = Cfg2<BN, EPI, true>::kSmem;
-  static_assert(kSmem <= 227 * 1024, "pair variant exceeds the shared memory of an SM");
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
-    if (e != cudaSuccess) return set_error(-2, "cudaFuncSetAttribute(gemm_tc2 pair): %s", cudaGetErrorString(e));
-    configured = true;
-  }
-  const long long tiles = static_cast<long long>((args.m_tiles + 1) / 2) * args.n_tiles;
-  const int pairs = num_sms() / 2;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(2 * static_cast<unsigned>(tiles < pairs ? tiles : pairs));
-  cfg.blockDim = dim3(Cfg2<BN, EPI, true>::kThreads);
-  cfg.dynamicSmemBytes = kSmem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = get_option(5) == 1 ? 1 : 0;
-  cfg.attrs = attr;
-  cfg.numAttrs = 2;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, maps, args);
-  if (e != cudaSuccess) return set_error(-2, "gemm_tc2 pair launch: %s", cudaGetErrorString(e));
-  return check_launch("gemm_tc2_pair");
-}
-
-template <int BN, int EPI, int ACT1, int ACT2, typename T>
 static int launch_variant2(const GemmMaps& maps, const GemmArgs& args, cudaStream_t stream) {
-  if constexpr (BN == 256) {
-    if (args.pair) return launch_pair2<BN, EPI, ACT1, ACT2, T>(maps, args, stream);
-  }
   auto kern = gemm_tc2_kernel<BN, EPI, ACT1, ACT2, T>;
+  using C = Cfg2<BN, EPI>;
   static bool configured_dev[64] = {};
   bool& configured = configured_dev[current_device_index()];
-  constexpr int kMaxSmem = (BN <= 64 && Cfg2<BN, EPI>::kSmemHalo > Cfg2<BN, EPI>::kSmem) ? Cfg2<BN, EPI>::kSmemHalo : Cfg2<BN, EPI>::kSmem;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmem);
     if (e != cudaSuccess) return set_error(-2, "cudaFuncSetAttribute(gemm_tc2): %s", cudaGetErrorString(e));
     configured = true;
   }
-  if (args.conv == 3 && (BN > 64 || args.halo_stages != Cfg2<BN, EPI>::kHaloStages))
-    return set_error(-3, "gemm_tc2: halo conv mode needs BLOCK_N <= 64");
   const long long tiles = static_cast<long long>(args.m_tiles) * args.n_tiles;
   const int sms = num_sms();
   const int grid = static_cast<int>(tiles < sms ? tiles : sms);
-  launch_pdl(kern, grid, Cfg2<BN, EPI>::kThreads, args.conv == 3 ? Cfg2<BN, EPI>::kSmemHalo : Cfg2<BN, EPI>::kSmem, stream, maps, args);
+  launch_pdl(kern, grid, C::kThreads, C::kSmem, stream, maps, args);
   return check_launch("gemm_tc2");
 }
 
@@ -1071,13 +710,6 @@ static int dispatch_epi(bool qkv, const GemmMaps& maps, const GemmArgs& args, cu
   } else {
     if (a1 == 0 && a2 == 0) return launch_variant2<BN, 0, 0, 0, T>(maps, args, stream);
     if (a1 == B2U_ACT_GELU && a2 == 0) {
-      if constexpr (BN == 256) {
-        // plain Linear -> GELU on CTA pairs (ViT fc1): the 16-warp lean epilogue
-        const b2u_epilogue& e = args.epi;
-        const bool lean = args.pair && args.conv == 0 && !e.residual && !e.add16 && !e.scale && !e.shift && e.ps_cout == 0 &&
-                          e.rows_in == 0 && args.N % 32 == 0 && get_option(6) == 0;
-        if (lean) return launch_pair2<BN, 4, B2U_ACT_GELU, 0, T>(maps, args, stream);
-      }
       return launch_variant2<BN, 0, B2U_ACT_GELU, 0, T>(maps, args, stream);
     }
     if (a1 == 0 && a2 == B2U_ACT_RELU) return launch_variant2<BN, 0, 0, B2U_ACT_RELU, T>(maps, args, stream);
@@ -1094,7 +726,6 @@ int gemm_v2_dispatch_t(bool qkv, int bn, const GemmMaps& maps, const GemmArgs& a
     case 32: return dispatch_epi<32, T>(qkv, maps, args, stream);
     case 64: return dispatch_epi<64, T>(qkv, maps, args, stream);
     case 128: return dispatch_epi<128, T>(qkv, maps, args, stream);
-    case 256: return dispatch_epi<256, T>(qkv, maps, args, stream);
     default: break;
   }
   return set_error(-3, "gemm_tc2: unsupported BLOCK_N %d", bn);

@@ -1,10 +1,10 @@
-// tcgen05 kind::tf32 GEMM for the TRAINING path: same parameter block, addressing modes and epilogue as b2u_f32_gemm
-// (csrc/fp32_tier.cu) - plain / transposed rows, the 3x3 window of an NHWC image on the A side (conv forward, conv data
-// gradient) or on the W side (conv weight gradient, K = output pixels), row remap, 2x2 pixel shuffle, split-K atomics -
-// but the products run on the 5th-generation tensor cores: fp32 operands rounded to TF32 (cvt.rna: 10 mantissa bits, the
-// mantissa width of the fp16 autocast the reference trains under, nnUNetTrainer.py:899-929, with fp32's exponent range),
-// fp32 accumulation in tensor memory.  The fp32 SIMT kernel stays the parity tier (1e-5); this one is the fast tier of
-// the train step (the SIMT GEMM was 87 % of it, profiles/r02_train_step_kernels_dinounet_b_b64.md).
+// TF32 tensor-core GEMM (sm_90a wgmma kind tf32) for the TRAINING path: same parameter block, addressing modes and epilogue
+// as b2u_f32_gemm (csrc/fp32_tier.cu) - plain / transposed rows, the 3x3 window of an NHWC image on the A side (conv
+// forward, conv data gradient) or on the W side (conv weight gradient, K = output pixels), row remap, 2x2 pixel shuffle,
+// split-K atomics - but the products run on the tensor cores: fp32 operands rounded to TF32 (cvt.rna: 10 mantissa bits,
+// the mantissa width of the fp16 autocast the reference trains under, nnUNetTrainer.py:899-929, with fp32's exponent
+// range), fp32 accumulation.  The fp32 SIMT kernel stays the parity tier (1e-5); this one is the fast tier of the train
+// step, whose time the SIMT GEMM dominates.
 //
 // Why register-path loaders instead of TMA: five of the eight operand modes are gathers that no tensor map expresses
 // without a transposed copy in HBM (A[k][m], W[k][n], flipped 3x3 weights, the per-pixel window with K = pixel index).
@@ -12,18 +12,22 @@
 // convolution gradients' row-contiguous operands 4 x 4 blocks (four LDG.128 along the rows, transposed in registers:
 // tf32::Roles in gemm_tf32_addr.h) - rounded to TF32 in registers and written to shared memory in exactly the layout a SWIZZLE_128B K-major tensor map would produce
 // (row r of a k-block = 128 B = 32 floats; 16-byte chunk c of row r lives at r*128 + ((c ^ (r & 7)) << 4)), so the
-// UMMA descriptors are byte-identical to the 16-bit GEMM's (make_desc_k128; +32 B per K = 8 step).
+// wgmma descriptors are the 16-bit GEMM's (make_gdesc_k128; +32 B per K = 8 step).
 //
-// CTA = one 128 x BN output tile of one K slice (grid = tiles (n fastest) x ksplit), 256 threads, 3-stage smem ring:
-//   all threads: wait stage free (tcgen05.commit -> mbarrier) -> st.shared the k-block fetched kPF iterations earlier ->
-//   fence.proxy.async -> issue the global loads of k-block kb + kPF into the freed register set (in flight across kPF
-//   barriers) -> __syncthreads -> one elected thread issues 4 x tcgen05.mma (M128, N = BN, K8) + commit.
-// Epilogue: tcgen05.ld, thread = accumulator row.  Two CTAs fit an SM's shared memory (60-96 KB each, BN TMEM columns).
+// CTA = one 128 x BN output tile of one K slice (grid = tiles (n fastest) x ksplit), 256 threads = two warpgroups of 64
+// tile rows each, 3-stage smem ring:
+//   all threads: st.shared the k-block fetched kPF iterations earlier -> fence.proxy.async -> issue the global loads of
+//   k-block kb + kPF into the freed register set (in flight across kPF barriers) -> __syncthreads -> each warpgroup issues
+//   4 x wgmma m64nBNk8 on its rows and waits until at most this k-block's group is in flight, so a stage is rewritten
+//   only after the MMAs of two iterations earlier have completed.
+// Epilogue: the accumulator fragments go through the (then idle) ring as a row-major fp32 tile, thread = accumulator row.
+// Two CTAs fit an SM's shared memory (60-96 KB each).
 #include <math.h>
 
 #include "common.cuh"
 #include "../../include/dinounet_b200.h"
 #include "gemm_tf32_addr.h"
+#include "wgmma.cuh"
 #include "host_util.h"
 
 namespace b2u {
@@ -45,8 +49,9 @@ template <int BN> struct TfCfg {
   static constexpr int kABytes = kTM * 128;
   static constexpr int kBBytes = BN * 128;
   static constexpr int kStage = kABytes + kBBytes;
-  static constexpr int kBarOff = kTStages * kStage;
-  static constexpr int kSmem = kBarOff + 64 + 1024;   // + barriers / TMEM slot + alignment slack
+  static constexpr int kAccRow = BN + 4;               // fp32 accumulator tile row stride (+16 B: conflict-free row reads)
+  static_assert(kTM * kAccRow * 4 <= kTStages * kStage, "the accumulator tile reuses the ring");
+  static constexpr int kSmem = kTStages * kStage + 1024;   // + alignment slack
 };
 
 __device__ __forceinline__ uint32_t to_tf32(float v) {
@@ -62,16 +67,6 @@ struct SmemPut {            // tf32::stage's sink: round to TF32, one 16-byte sh
                  : "memory");
   }
 };
-__device__ __forceinline__ void tc_mma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
 
 // ABLK / WBLK: staging shape of the two operands (tf32::pick_modes), compile-time so that each instantiation carries only
 // its own loader (a runtime switch cost the row-mode shapes 6-15 %)
@@ -86,34 +81,22 @@ __global__ void __launch_bounds__(kTThreads, B2U_TF32_MINB) gemm_tf32_kernel(con
 
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const uint32_t smem_base = smem_u32(smem);
-  uint64_t* empty_bar = reinterpret_cast<uint64_t*>(smem + C::kBarOff);   // [kTStages]
-  uint64_t* done_bar = empty_bar + kTStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(done_bar + 1);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wg = warp >> 2;                            // MMA: tile rows [64 wg, 64 wg + 64)
   long long m0;
   int n0;
   tile_origin(p, BN, static_cast<long long>(blockIdx.x), m0, n0);
 
-  if (tid == 0) {
-    for (int s = 0; s < kTStages; ++s) mbar_init(&empty_bar[s], 1);
-    mbar_init(done_bar, 1);
-    fence_mbar_init();
-  }
-  if (warp == 0) { tmem_alloc(tmem_slot, BN); tmem_relinquish(); }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
   const Roles R = make_roles(p, tid, m0, n0, BN, ABLK, WBLK);   // this thread's rows / chunks of the two operand tiles
   constexpr int kWN = BN / 32;
-  constexpr uint32_t idesc = make_idesc_f16(2 /* TF32 */, kTM, BN);
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
 
   // kPF register sets: k-block kb lives in set kb % kPF from the moment its loads are issued (kPF iterations ahead) until it
-  // is stored to the ring.  MEASURED (same box, 15 shapes, profiles/r02_tf32_gemm_micro.md): kPF 1 / 2 / 3 at two CTAs per SM
-  // = 32.9 / 37.4 / 42.6 ms in total - deeper prefetch LOSES: the kernel is bound by L2->SM operand bytes (3.7 TB/s at the
-  // 768-wide linears = 32 FLOP per operand byte of a 128 x 128 fp32 tile), not by load latency; default 1.
+  // is stored to the ring.  Default 1: the kernel is bound by L2->SM operand bytes (32 FLOP per operand byte of a 128 x 128
+  // fp32 tile), not by load latency, and deeper prefetch costs registers at two CTAs per SM.
   float4 ra[kPF][4], rw[kPF][4];
 #pragma unroll
   for (int u = 0; u < kPF; ++u) {
@@ -127,59 +110,55 @@ __global__ void __launch_bounds__(kTThreads, B2U_TF32_MINB) gemm_tf32_kernel(con
     for (int u = 0; u < kPF; ++u) {
       const int kb = kb0 + u;
       if (kb >= nkb) break;                            // uniform over the CTA
-      const int s = kb % kTStages;
-      if (kb >= kTStages) mbar_wait(&empty_bar[s], static_cast<uint32_t>((kb / kTStages - 1) & 1));   // MMAs of k-block kb - 3 have read the stage
+      const int s = kb % kTStages;                     // free: every warpgroup has waited for the MMAs of k-block kb - 2
       const uint32_t sbase = smem_base + static_cast<uint32_t>(s) * C::kStage;
       stage<ABLK, 4>(R.a_r, R.a_c0, true, ra[u], SmemPut{sbase});
       stage<WBLK, kWN>(R.w_r, R.w_c0, R.w_n != 0, rw[u], SmemPut{sbase + C::kABytes});
-      fence_proxy_async();                             // generic-proxy writes -> visible to the tensor core's async proxy
+      fence_proxy_async();                             // generic-proxy writes -> visible to the wgmma async proxy
       if (kb + kPF < nkb) {                            // refill this register set: in flight across kPF barriers / MMA issues
         fetch_a<ABLK>(p, R, k_lo + (kb + kPF) * kTK, k_hi, ra[u]);
         fetch_w<WBLK, kWN>(p, R, k_lo + (kb + kPF) * kTK, k_hi, rw[u]);
       }
       __syncthreads();
-      if (warp == 0) {
-        if (elect_one()) {
-          tc_fence_after();
-          const uint64_t da = make_desc_k128(sbase);
-          const uint64_t db = make_desc_k128(sbase + C::kABytes);
+      {
+        const uint64_t da = make_gdesc_k128(sbase + static_cast<uint32_t>(wg * 64 * 128));
+        const uint64_t db = make_gdesc_k128(sbase + C::kABytes);
+        wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < kTK / 8; ++k)
-            tc_mma_tf32(tmem_base, da + static_cast<uint64_t>(k * 2), db + static_cast<uint64_t>(k * 2), idesc, (kb | k) != 0 ? 1u : 0u);
-          tc_commit(&empty_bar[s]);
-          if (kb == nkb - 1) tc_commit(done_bar);      // everything issued so far has completed when this one arrives
-        }
-        __syncwarp();
+        for (int k = 0; k < kTK / 8; ++k)
+          wgmma_ss<2, BN>(acc, da + static_cast<uint64_t>(k * 2), db + static_cast<uint64_t>(k * 2), (kb | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();
       }
     }
   }
 
   // ---------------------------------------------------------------- epilogue: thread = accumulator row
-  mbar_wait(done_bar, 0);
-  tc_fence_after();
+  wgmma_wait<0>();
+  __syncthreads();                                     // every MMA has read its stage: the ring holds the accumulator tile
+  float* s_acc = reinterpret_cast<float*>(smem);       // [kTM][kAccRow]
   {
-    const int q = warp & 3, half = warp >> 2;          // TMEM lane quarter (fixed by warp % 4), column half
-    constexpr int kCols = BN / 2;
-    const EpiRow e = make_epi_row(p, m0 + q * 32 + lane);
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(half * kCols);
-#pragma unroll 1
-    for (int c0 = 0; c0 < kCols; c0 += 16) {
-      uint32_t v[16];
-      tmem_ld16(taddr + static_cast<uint32_t>(c0), v);   // .sync.aligned: every lane, also rows beyond M
-      tmem_ld_wait();
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        const float acc[4] = {__uint_as_float(v[g * 4]), __uint_as_float(v[g * 4 + 1]), __uint_as_float(v[g * 4 + 2]), __uint_as_float(v[g * 4 + 3])};
-        emit4(p, e, n0 + half * kCols + c0 + g * 4, acc);
-      }
-      __syncwarp();                                      // reconverge before the next warp-collective tcgen05.ld
+    for (int j = 0; j < BN / 8; ++j) {
+      const int c = 8 * j + 2 * (lane & 3);
+      *reinterpret_cast<float2*>(s_acc + r0 * C::kAccRow + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(s_acc + (r0 + 8) * C::kAccRow + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
     }
   }
-  tc_fence_before();
   __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, BN);
+  {
+    const int q = warp & 3, half = warp >> 2;          // rows [32 q, 32 q + 32), column half
+    constexpr int kCols = BN / 2;
+    const int row = q * 32 + lane;
+    const EpiRow e = make_epi_row(p, m0 + row);
+    const float* src = s_acc + row * C::kAccRow + half * kCols;
+#pragma unroll 1
+    for (int c0 = 0; c0 < kCols; c0 += 4) {
+      const float4 v = *reinterpret_cast<const float4*>(src + c0);
+      const float a4[4] = {v.x, v.y, v.z, v.w};
+      emit4(p, e, n0 + half * kCols + c0, a4);
+    }
   }
 }
 

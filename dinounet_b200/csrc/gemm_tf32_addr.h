@@ -1,9 +1,9 @@
-// Addressing of the tcgen05 kind::tf32 GEMM (gemm_tf32.cu), as host/device inline functions: which operand element every
+// Addressing of the TF32 wgmma GEMM (gemm_tf32.cu), as host/device inline functions: which operand element every
 // loader thread fetches in every mode of b2u_f32_gemm_params, where it lands in the 128B-swizzled k-block tile, how the
 // K range is sliced, and where an accumulator element goes in the epilogue.  The kernel is the composition of these
-// functions with the tcgen05 / mbarrier plumbing; tests/test_tf32_gemm_hostsim_cpu.py compiles the SAME functions for the
+// functions with the wgmma plumbing; tests/test_tf32_gemm_hostsim_cpu.py compiles the SAME functions for the
 // host (csrc/gemm_tf32_hostsim.cpp: a software model of the 256 threads of a CTA + the SWIZZLE_128B K-major read-out of
-// tcgen05.mma) and checks every mode against torch without a GPU.
+// the MMA) and checks every mode against torch without a GPU.
 #pragma once
 #include <math.h>
 #include <stdint.h>
@@ -46,8 +46,8 @@ struct Row {              // what one loader thread knows about "its" operand ro
 //   block mode (operand contiguous along its ROW index: A[k][m], W[k][n], the flipped 3x3 weights, the pixel-indexed window
 //              of a weight gradient): a 4 x 4 block = 4 consecutive rows x one chunk, fetched as four LDG.128 ALONG THE ROWS
 //              (one per k) and transposed in registers into the four 16-byte chunks the K-major tile wants.  Row mode needs
-//              16 scalar loads with 16 address computations for the same 16 elements: the weight-gradient GEMMs were bound
-//              by exactly that integer work (15 TF/s at 1.3 TB/s of L2->SM traffic, profiles/r02_tf32_gemm_micro.md).
+//              16 scalar loads with 16 address computations for the same 16 elements, integer work that bounds the
+//              weight-gradient GEMMs.
 struct Roles {
   int amode, stride, Ho, Wo;
   bool a_blk, w_blk;
@@ -99,9 +99,9 @@ TF_HD float window(const float* img, int Hin, int Win, int Cc, int stride, int c
 
 // Which staging shape each operand gets.  Block mode needs the row-contiguous addressing AND 16-byte alignment of every row
 // group; it is used for the CONVOLUTION gradients only (weight gradient: both operands; data gradient: the flipped weights):
-// measured on B200 (profiles/r02_tf32_gemm_micro.md) it doubles the 3x3 weight gradients (4.9 -> 2.6 ms at 512^2 64->32,
-// B = 8) and speeds up the data gradients by 7-30 %, while the plain linears' transposed operands (small, L2-resident
-// weight / dy^T slices) ran 10-30 % slower in block mode than with scalar row-mode loads.
+// block mode replaces 16 scalar loads and address computations per 4 x 4 block by four 16-byte loads, which is what the
+// 3x3 weight and data gradients are bound by; the plain linears' transposed operands are small, L2-resident weight / dy^T
+// slices, for which scalar row-mode loads are kept.
 TF_HD void pick_modes(const b2u_f32_gemm_params& p, bool& a_blk, bool& w_blk) {
   const bool a_al = (reinterpret_cast<uintptr_t>(p.A) & 15) == 0, w_al = (reinterpret_cast<uintptr_t>(p.W) & 15) == 0;
   w_blk = p.conv != 0 && w_al &&

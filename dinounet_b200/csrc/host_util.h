@@ -20,11 +20,9 @@ int get_option(int key);
 
 // Programmatic dependent launch (PDL), OPT-IN (option 5 = 1): every kernel of the forward plan can be launched with
 // cudaLaunchAttributeProgrammaticStreamSerialization; each calls `griddepcontrol.wait` before it touches global memory
-// (after its barrier-init / TMEM-alloc / tensormap-prefetch prologue where it has one) and the persistent GEMM / attention
-// kernels call `griddepcontrol.launch_dependents` when a CTA has finished its tiles.  MEASURED on B200 (same box, A/B/A/B,
-// dinounet_l B=32, graph replay): trigger at kernel start 50.1 vs 48.3 ms/step, trigger at CTA end 49.6 vs 48.4 - PDL LOSES
-// 2.4-3.6 % here (the plan's kernels are persistent with ~200 KB shared memory each, so a dependent cannot become resident
-// before its predecessor's CTAs exit, and the programmatic edges cost more than the ~3 us launch gaps they hide).  Default off;
+// (after its barrier-init / tensormap-prefetch prologue where it has one) and the persistent GEMM / attention
+// kernels call `griddepcontrol.launch_dependents` when a CTA has finished its tiles.  Default off (the plan's persistent
+// kernels hold most of an SM's shared memory, so a dependent cannot become resident before its predecessor's CTAs exit);
 // with the attribute off `griddepcontrol.wait` is a no-op.
 template <typename... KArgs, typename... Args>
 static inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {

@@ -1,4 +1,4 @@
-// MultiScaleDeformableAttention forward for sm_100a.
+// MultiScaleDeformableAttention forward for sm_90a.
 //
 // b2u_msda_forward — the hot-path kernel: one warp per query, lane = (head = lane/2, channel half = lane&1).  The
 //   per-head prologue the reference runs as separate torch ops (softmax over the points, reference point + offset /
@@ -201,7 +201,7 @@ static int launch_msda_smem(const void* value, const float* offaw, void* out, in
     configured = smem;
   }
   const int groups = heads / HPC;
-  // enough CTAs for several waves of (CTAs that fit an SM) x 148 SMs; each re-stages its slab from L2
+  // enough CTAs for several waves of (CTAs that fit an SM) x 132 SMs; each re-stages its slab from L2
   const int per_sm = static_cast<int>(std::min<size_t>(8, std::max<size_t>(1, (200 * 1024) / std::max<size_t>(smem, 1))));
   int qsplit = ((per_sm > 1 ? 6 : 2) * per_sm * num_sms() + B * groups - 1) / (B * groups);
   if (qsplit < 1) qsplit = 1;

@@ -1,5 +1,5 @@
 """Forward engine: packs a Dino U-Net state dict into kernel-native layouts and runs the forward as a fixed launch
-plan of hand-written sm_100a kernels (through the C-ABI in include/dinounet_b200.h).
+plan of hand-written sm_90a kernels (through the C-ABI in include/dinounet_b200.h).
 
 Data layout in HBM (everything channels-last / token-major, C contiguous):
   * ViT residual stream X  [B*ntok, D] fp32; GEMM operands (LN outputs, q/k/v [B,H,ntok,64], attention out, MLP hidden)
@@ -66,7 +66,7 @@ class ForwardEngine:
         if self.hd not in (64, 128) or self.v.ffn_layer not in ("mlp", "swiglu64"):
             raise NotImplementedError(f"{variant}: kernels exist for head_dim 64/128 and mlp / swiglu64 FFNs")
         if attn_impl != "tc":
-            raise NotImplementedError("the only attention kernel is the tcgen05 / TMEM one (attn_impl='tc'); the first-generation "
+            raise NotImplementedError("the only attention kernel is the wgmma one (attn_impl='tc'); the first-generation "
                                       "mma.sync kernel was removed in round 2")
         if tuple(features) != (32, 64, 128, 256):
             raise NotImplementedError("kernels are built for the planner's features_per_stage=(32,64,128,256)")
@@ -85,7 +85,7 @@ class ForwardEngine:
         else:
             self.tv, self.tr = _TORCH16[self.vt], _TORCH16[self.rt]
         self.features = tuple(features)
-        self.attn_impl = attn_impl   # "tc" = tcgen05/TMEM kernel
+        self.attn_impl = attn_impl   # "tc" = wgmma flash-attention kernel
         # The adapter's query stream c [B, 5376, D] (dinov3_adapter.py:210-231).  "fp32" (default) = the reference's dtype
         # under autocast: the 16-bit SPM outputs are promoted to fp32 by `c + level_embed` (fp32 parameter) and stay fp32
         # through `query + attn`.  "16" = opt-in: stored in rest_dtype, every residual update rounded to 16 bits (half the

@@ -158,7 +158,7 @@ def load() -> C.CDLL:
         if not os.path.exists(_LIB_PATH):
             raise NativeLibraryError(
                 f"{_LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a). dinounet_b200 has no CPU or PyTorch fallback.")
+                "(nvcc, sm_90a). dinounet_b200 has no CPU or PyTorch fallback.")
         try:
             lib = C.CDLL(_LIB_PATH)
         except OSError as e:  # pragma: no cover

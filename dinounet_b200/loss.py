@@ -1,4 +1,4 @@
-"""Dice + cross-entropy loss and the online-validation statistics on the logits of the B200 forward path.
+"""Dice + cross-entropy loss and the online-validation statistics on the logits of the native forward path.
 
 Mirror of the reference objects the trainer builds and calls (nnUNetTrainer.py:363-365, :961-1005):
 `DC_and_CE_loss(soft_dice_kwargs, ce_kwargs, weight_ce, weight_dice, ignore_label, dice_class)` with the same
@@ -76,9 +76,9 @@ class DC_and_CE_loss(nn.Module):
                  dice_class=None):
         super().__init__()
         if ignore_label is not None:
-            raise NotImplementedError("ignore_label is not covered by the fused B200 loss")
+            raise NotImplementedError("ignore_label is not covered by the fused native loss")
         if ce_kwargs:
-            raise NotImplementedError(f"cross-entropy options {sorted(ce_kwargs)} are not covered by the fused B200 loss")
+            raise NotImplementedError(f"cross-entropy options {sorted(ce_kwargs)} are not covered by the fused native loss")
         kw = dict(soft_dice_kwargs)
         self.batch_dice = bool(kw.pop("batch_dice", False))
         self.do_bg = bool(kw.pop("do_bg", True))
@@ -86,7 +86,7 @@ class DC_and_CE_loss(nn.Module):
         self.ddp = bool(kw.pop("ddp", True))
         kw.pop("apply_nonlin", None)
         if kw:
-            raise NotImplementedError(f"soft dice options {sorted(kw)} are not covered by the fused B200 loss")
+            raise NotImplementedError(f"soft dice options {sorted(kw)} are not covered by the fused native loss")
         self.weight_dice = weight_dice
         self.weight_ce = weight_ce
         self.ignore_label = None
@@ -95,7 +95,7 @@ class DC_and_CE_loss(nn.Module):
     def _run(self, net_output, target):
         if self.batch_dice and self.ddp and torch.distributed.is_available() and torch.distributed.is_initialized() \
                 and torch.distributed.get_world_size() > 1:
-            raise NotImplementedError("DDP batch-dice (all-gather of the dice sums) is not covered by the fused B200 loss")
+            raise NotImplementedError("DDP batch-dice (all-gather of the dice sums) is not covered by the fused native loss")
         loss, out3, counts, bad = _DiceCE.apply(net_output, target, self.weight_ce, self.weight_dice, self.batch_dice,
                                                 self.do_bg, self.smooth)
         if self.check_labels and int(bad.item()):

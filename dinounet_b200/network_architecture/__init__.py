@@ -1,4 +1,4 @@
-"""`dinounet.network_architecture`-style module surface of the B200-native Dino U-Net (see modules.py)."""
+"""`dinounet.network_architecture`-style module surface of the native Dino U-Net (see modules.py)."""
 from .modules import (  # noqa: F401
     DinoUNet, DINOv3EncoderAdapter, FAPM, SqueezeExcitation, DepthwiseSeparableConv, LearnableUpsampleBlock,
     UNetDecoder, DINOv3_Adapter, SpatialPriorModule, InteractionBlockWithCls, Extractor, ConvFFN, DWConv,

@@ -15,7 +15,7 @@ keys: `decoder.encoder.*` and `...convs.N.all_modules.M.*`) as
   dynamic_network_architectures   StackedConvBlocks / ConvDropoutNormReLU (third party, restated)
 
 These classes OWN the parameters (so checkpoints, optimizers, `.to()`, `.eval()` behave as with the reference) but hold
-no PyTorch compute: the only `forward` is `DinoUNet.forward`, which runs the sm_100a kernel plan of
+no PyTorch compute: the only `forward` is `DinoUNet.forward`, which runs the sm_90a kernel plan of
 `dinounet_b200.engine.ForwardEngine` over packed copies of these parameters (re-packed after `load_state_dict` / `.to`).
 """
 from __future__ import annotations
@@ -36,7 +36,7 @@ from .. import config as cfg
 class _NoForward(nn.Module):
     def forward(self, *a, **k):  # pragma: no cover
         raise RuntimeError(f"{type(self).__name__} is a parameter container; run the model through DinoUNet.forward "
-                           "(hand-written sm_100a kernels) - there is no PyTorch fallback path")
+                           "(hand-written sm_90a kernels) - there is no PyTorch fallback path")
 
 
 # ----------------------------------------------------------------------------------------------- DINOv3 ViT
@@ -445,7 +445,7 @@ class UNetDecoder(_NoForward):
         assert len(n_conv_per_stage) == n_enc - 1, "n_conv_per_stage must have as many entries as we have " \
                                                    "resolution stages - 1 (n_stages in encoder - 1), here: %d" % n_enc
         if encoder.conv_op is not nn.Conv2d:
-            raise NotImplementedError("the B200 forward path is 2D (conv_op=Conv2d), as forced by main_dinov3")
+            raise NotImplementedError("the native forward path is 2D (conv_op=Conv2d), as forced by main_dinov3")
         conv_bias = encoder.conv_bias if conv_bias is None else conv_bias
         norm_op = encoder.norm_op if norm_op is None else norm_op
         norm_op_kwargs = encoder.norm_op_kwargs if norm_op_kwargs is None else norm_op_kwargs
@@ -488,7 +488,7 @@ def load_dinov3_model(model_name: str, pretrained_path: str = None) -> DinoVisio
 
 
 class DinoUNet(nn.Module):
-    """U-Net with DINOv3_Adapter as encoder (dinounet_training.py:632-829), forward on hand-written sm_100a kernels."""
+    """U-Net with DINOv3_Adapter as encoder (dinounet_training.py:632-829), forward on hand-written sm_90a kernels."""
 
     #: 16-bit types of the kernel path: ViT GEMMs / everything else (the reference's inner bf16 / outer fp16 autocast)
     vit_dtype = "bf16"
@@ -500,7 +500,7 @@ class DinoUNet(nn.Module):
     #: "16" = the bf16/fp16 tensor-core kernels (default, benchmarked); "fp32" = the fp32 parity tier (plain SIMT kernels,
     #: within 1e-5 of the reference's fp32 forward; set before the first forward or call repack())
     precision = "16"
-    #: matrix products of the TRAINING step's trainable part: "tf32" = tcgen05 tensor cores, TF32-rounded operands, fp32
+    #: matrix products of the TRAINING step's trainable part: "tf32" = wgmma tensor cores, TF32-rounded operands, fp32
     #: accumulation (default; the reference trains under fp16 autocast = the same mantissa); "fp32" = IEEE-fp32 SIMT kernels
     #: (the tier the gradient goldens are held to at 2e-3)
     train_gemm = "tf32"
@@ -629,7 +629,7 @@ class DinoUNet(nn.Module):
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         if self.decoder.deep_supervision:
-            raise NotImplementedError("deep supervision outputs are not produced by the B200 forward path "
+            raise NotImplementedError("deep supervision outputs are not produced by the native forward path "
                                       "(DinoUNetTrainer derives from nnUNetTrainerNoDeepSupervision)")
         if torch.is_grad_enabled() and self.training:
             # training step (nnUNetTrainer.py:899-929): frozen ViT on the engine, everything else differentiable through the

@@ -1,4 +1,4 @@
-"""Sliding-window prediction on the B200 forward engine (SURVEY.md section 8f rank 1).
+"""Sliding-window prediction on the native forward engine (SURVEY.md section 8f rank 1).
 
 Mirror of the reference's `nnUNetPredictor` sliding-window surface (inference/predict_from_raw_data.py:39-64,
 132-146, 502-553, 572-621, 680-726) and of `inference/sliding_window_prediction.py:11-61`:
@@ -170,7 +170,7 @@ class SlidingWindowPredictor:
         net.eval()
         patch = [int(p) for p in self.configuration_manager.patch_size]
         if len(patch) != 2 or patch[0] != patch[1]:
-            raise NotImplementedError("the B200 engine runs square 2D patches (main_dinov3 forces 512x512)")
+            raise NotImplementedError("the native engine runs square 2D patches (main_dinov3 forces 512x512)")
         lib = L.load()
         dev = self.device if self.device.index is not None else torch.device("cuda", torch.cuda.current_device())
         heads = int(self.label_manager.num_segmentation_heads)

@@ -12,7 +12,7 @@ head (289 tensors).  Here:
     is used as the tape only: what it executes itself is data movement (views, cat, contiguous) and gradient accumulation
     for tensors with several consumers;
   * the matrix products (F.linear / Conv2d / ConvTranspose2d: forward, data gradient, weight gradient) have two tiers
-    with ONE parameter block: `gemm="tf32"` (default) = `b2u_tf32_gemm`, tcgen05 tensor cores with TF32-rounded operands
+    with ONE parameter block: `gemm="tf32"` (default) = `b2u_tf32_gemm`, wgmma tensor cores with TF32-rounded operands
     and fp32 accumulation (the mantissa of the fp16 autocast the reference trains under); `gemm="fp32"` = `b2u_f32_gemm`,
     the IEEE-fp32 SIMT kernel the gradient goldens are held to at 2e-3.  Everything else is fp32 in both tiers;
   * semantics = the gradient oracle's (oracle/grad_oracle.py, pinned to autograd through the REAL reference): eval-mode

@@ -2,7 +2,7 @@
 
 Mirrors `DinoUNetTrainer` and its four subclasses (dinounet_training.py:833-930): `set_network_config` stores the
 planner's architecture dict on the class, and the static `build_network_architecture` hook
-(nnUNetTrainer.py:265-298) returns the B200-native `DinoUNet`.  When the reference's nnU-Net package is importable the
+(nnUNetTrainer.py:265-298) returns the native `DinoUNet`.  When the reference's nnU-Net package is importable the
 trainers derive from its `nnUNetTrainerNoDeepSupervision`, so `api.training(trainer_class=DinoUNetTrainer_l, ...)`
 works unchanged; otherwise they derive from `object` (the hook itself is a staticmethod and needs no base class).
 """
@@ -58,14 +58,14 @@ class DinoUNetTrainer(_Base):
     # ---- forward-only callers of the path that the trainer owns (nnUNetTrainer.py:355-365, :945-1005)
     def _build_loss(self):
         """Label-map training: Dice (batch_dice from the plans, smooth 1e-5, no background) + CE, weights 1:1 — the
-        fused B200 loss.  No deep-supervision wrapper (the trainer derives from nnUNetTrainerNoDeepSupervision)."""
+        fused native loss.  No deep-supervision wrapper (the trainer derives from nnUNetTrainerNoDeepSupervision)."""
         if self.label_manager.has_regions:
-            raise NotImplementedError("region-based (sigmoid/BCE) training is not covered by the fused B200 loss")
+            raise NotImplementedError("region-based (sigmoid/BCE) training is not covered by the fused native loss")
         return DC_and_CE_loss({"batch_dice": self.configuration_manager.batch_dice, "smooth": 1e-5, "do_bg": False,
                                "ddp": self.is_ddp}, {}, weight_ce=1, weight_dice=1,
                               ignore_label=self.label_manager.ignore_label)
 
-    # ---- training step on the B200 path (nnUNetTrainer.py:486-489, 899-929)
+    # ---- training step on the native path (nnUNetTrainer.py:486-489, 899-929)
     def configure_optimizers(self):
         """SGD(momentum 0.99, nesterov, weight decay) + the reference's PolyLRScheduler (it only writes param_groups[0]['lr'])
         on the fused kernels; gradient clipping (12) is part of the fused step."""
@@ -90,7 +90,7 @@ class DinoUNetTrainer(_Base):
         return {"loss": loss.cpu().numpy()}
 
     def validation_step(self, batch: dict) -> dict:
-        """One online-validation batch: B200 forward, then loss + hard tp/fp/fn in one fused pass over the logits."""
+        """One online-validation batch: native forward, then loss + hard tp/fp/fn in one fused pass over the logits."""
         data = batch["data"].to(self.device, non_blocking=True)
         target = batch["target"]
         if isinstance(target, list):
@@ -126,7 +126,7 @@ DINOV3_TRAINERS = {"dinounet_s": DinoUNetTrainer_s, "dinounet_b": DinoUNetTraine
                    "dinounet_7b": DinoUNetTrainer_7b}
 
 
-_DISCOVERABLE_STUB = '''"""Makes the B200-native Dino U-Net trainers visible to nnU-Net's name-based trainer lookup.
+_DISCOVERABLE_STUB = '''"""Makes the native Dino U-Net trainers visible to nnU-Net's name-based trainer lookup.
 
 `recursive_find_python_class` (dinounet/utilities/find_class_by_name.py:7-24) walks dinounet/training/nnUNetTrainer/*.py;
 the reference's own `DinoUNetTrainer_*` classes live in the top-level script dinounet_training.py and are therefore

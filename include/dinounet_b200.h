@@ -1,6 +1,6 @@
-/* dinounet_b200 — C-ABI of the B200-native Dino U-Net forward path.
+/* dinounet_b200 — C-ABI of the H100-native Dino U-Net forward path.
  *
- * Plain pointers and sizes only (no torch types).  Every function launches hand-written sm_100a kernels on the
+ * Plain pointers and sizes only (no torch types).  Every function launches hand-written sm_90a kernels on the
  * given CUDA stream, never allocates, never synchronises, and returns 0 on success or a negative error code
  * (message via b2u_last_error()).  All device tensors are channels-last ("token-major"): [rows, C] with C contiguous.
  *
@@ -57,7 +57,7 @@ typedef struct b2u_epilogue {
   int64_t ldadd;
 } b2u_epilogue;
 
-/* tcgen05 tensor-core GEMM / implicit-GEMM 3x3 convolution:  acc[M, N] = A[M, K] * Wp[N, K]^T.
+/* wgmma tensor-core GEMM / implicit-GEMM 3x3 convolution:  acc[M, N] = A[M, K] * Wp[N, K]^T.
  * conv == NONE : A is [M, K] row-major (row stride lda).  Replaces F.linear / 1x1 Conv2d / ConvTranspose2d(k2,s2)
  *                (attention.py:88-90, ffn_layers.py:43-49, ms_deform_attn.py:183-215, dinov3_adapter.py:274-277,467,
  *                dinounet_training.py:419-441,255-264,613).
@@ -105,10 +105,10 @@ typedef struct b2u_qkv_params {
 
 int b2u_qkv_rope(const b2u_qkv_params* p, b2u_stream_t stream);
 
-/* tcgen05 / TMEM flash attention, non-causal softmax attention (attention.py:106-118 -> F.scaled_dot_product_attention):
+/* wgmma flash attention, non-causal softmax attention (attention.py:106-118 -> F.scaled_dot_product_attention):
  * q,k [B, heads, ntok, 64], vt = V^T [B, heads, 64, npad]
  * with zero padding columns (see b2u_qkv_params.v_transposed) -> out [B, ntok, heads*64].  Only the query rows
- * [q_begin, ntok) are produced (128-row tiles, two per work item); keys always span [0, ntok).  With q_begin = the
+ * [q_begin, ntok) are produced (128-row tiles, one per CTA); keys always span [0, ntok).  With q_begin = the
  * number of cls/storage tokens the ViT's 1024 patch rows fill whole tiles and b2u_attention_rows does the prefix. */
 int b2u_attention_tc(const void* q, const void* k, const void* vt, void* out, int32_t B, int32_t heads, int32_t ntok,
                      int32_t npad, int32_t q_begin, float scale, int32_t dtype, b2u_stream_t stream);
@@ -266,16 +266,10 @@ int b2u_seg_head(const void* x, const float* sums, const float* gamma, const flo
 /* cudaMemsetAsync(ptr, 0, bytes) on the stream (statistics accumulators must be zeroed every forward). */
 int b2u_zero(void* ptr, int64_t bytes, b2u_stream_t stream);
 
-/* Tuning / A-B switches.  key 0 (B2U_OPT_GEMM_IMPL): 0 = persistent 128x256-tile tcgen05 kernel (default),
- * 1 = the first-generation one-tile-per-CTA kernel. */
-/* key 1 (B2U_OPT_MSDA_IMPL): 0 = shared-memory value-slab gather (default), 1 = first-generation warp-per-query kernel. */
-/* key 2 (B2U_OPT_CONV_HALO): 0 = 3x3 convs with <= 64 in/out channels and >= 128-px rows use the halo-reuse mode
- * (default), 1 = always the per-tap TMA walk. */
-/* key 3 (B2U_OPT_GEMM_PAIR): 0 = plain GEMMs with 256-wide tiles run on CTA pairs (tcgen05 cta_group::2, 256 x 256
- * tile per pair, each CTA stages half of the weight tile) (default), 1 = one CTA per tile. */
-/* key 4 (B2U_OPT_ATTN_SPLIT): 0 = two softmax warps per (query tile, TMEM lane quarter), each owning half of the key
- * columns / head dims (default), 1 = one warp. */
-enum { B2U_OPT_GEMM_IMPL = 0, B2U_OPT_MSDA_IMPL = 1, B2U_OPT_CONV_HALO = 2, B2U_OPT_GEMM_PAIR = 3, B2U_OPT_ATTN_SPLIT = 4 };
+/* Tuning / A-B switches (b2u_set_option).  key 1 (B2U_OPT_MSDA_IMPL): 0 = shared-memory value-slab gather (default),
+ * 1 = first-generation warp-per-query kernel.  key 5: 1 = programmatic dependent launch across the plan (default off).
+ * key 7: 1 = no L2 prefetch of the next tile's residual rows in short-K GEMMs (default on). */
+enum { B2U_OPT_MSDA_IMPL = 1 };
 /* ---------------------------------------------------------------------------------------------------------------
  * fp32 parity tier (csrc/fp32_tier.cu): the same forward in IEEE fp32 with plain SIMT kernels, selected by
  * `DinoUNet.precision = "fp32"`.  It is the path held to north_star's 1e-5 against the reference's fp32 (CPU) forward;
@@ -313,7 +307,7 @@ typedef struct b2u_f32_gemm_params {
 int b2u_f32_gemm(const b2u_f32_gemm_params* p, b2u_stream_t stream);   /* F.linear / Conv2d 1x1, 3x3 / ConvTranspose2d k2 s2 */
 /* Same parameter block, addressing modes and epilogue on the tensor cores (csrc/gemm_tf32.cu): operands rounded to TF32
  * (round-to-nearest, 10 mantissa bits = the fp16 autocast the reference trains under, nnUNetTrainer.py:899-929, with fp32's
- * exponent range), fp32 accumulation in tensor memory (tcgen05.mma kind::tf32).  The fast tier of the TRAINING step's
+ * exponent range), fp32 accumulation (wgmma kind tf32).  The fast tier of the TRAINING step's
  * matrix products (forward, data gradient, weight gradient of F.linear / Conv2d / ConvTranspose2d); not bit-comparable
  * with b2u_f32_gemm (about 1e-3 relative per product). */
 int b2u_tf32_gemm(const b2u_f32_gemm_params* p, b2u_stream_t stream);

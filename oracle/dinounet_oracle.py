@@ -2,7 +2,7 @@
 
 A functional, pure-PyTorch CPU restatement of the reference's Dino U-Net *forward* path,
 written against a flat state dict that uses the reference's own parameter names.  It is
-the checker for the hand-written sm_100a kernels; only `tests/`, `__graft_entry__.smoke()`
+the checker for the hand-written sm_90a kernels; only `tests/`, `__graft_entry__.smoke()`
 and `bench.py`'s cpu_baseline / `--impl reference` legs may import it.
 
 Parity pin: `tests/test_oracle_vs_reference.py` (runs where /root/reference exists) asserts

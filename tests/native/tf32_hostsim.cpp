@@ -1,10 +1,10 @@
 // Host model of gemm_tf32_kernel (dinounet_b200/csrc/gemm_tf32.cu) for the CPU test suite: the kernel's own addressing
 // functions (csrc/gemm_tf32_addr.h, compiled for the host) are executed for all 256 threads of every CTA, writing the
 // 128B-swizzled k-block tiles into a byte array that stands for shared memory; the tensor core is modelled by reading those
-// tiles back the way tcgen05.mma reads a K-major SWIZZLE_128B operand (row r, element k of the k-block at byte
-// r*128 + k*4 with address bits [4,7) XORed by bits [7,10)), accumulating in double; the epilogue walks the TMEM lane /
+// tiles back the way the tensor-core MMA reads a K-major SWIZZLE_128B operand (row r, element k of the k-block at byte
+// r*128 + k*4 with address bits [4,7) XORed by bits [7,10)), accumulating in double; the epilogue walks the accumulator-tile row /
 // column assignment of the 8 warps.  What this does NOT model: descriptors, barriers, the hardware itself - those are
-// checked by tests/test_gpu_tf32_gemm.py on a B200.  Test infrastructure only.
+// checked by tests/test_gpu_tf32_gemm.py on the GPU.  Test infrastructure only.
 #include <stdint.h>
 #include <stdlib.h>
 #include <string.h>

@@ -107,7 +107,7 @@ def test_no_cpu_fallback(built):
 
 def test_engine_rejects_unsupported_kernel_choices(built):
     from dinounet_b200.engine import ForwardEngine
-    with pytest.raises(NotImplementedError):   # the tcgen05 attention kernel is the only one
+    with pytest.raises(NotImplementedError):   # the wgmma attention kernel is the only one
         ForwardEngine("dinounet_7b", {}, 2, torch.device("cpu"), attn_impl="mma")
     with pytest.raises(ValueError):
         ForwardEngine("dinounet_xl", {}, 2, torch.device("cpu"))
@@ -115,7 +115,7 @@ def test_engine_rejects_unsupported_kernel_choices(built):
 
 def test_training_checkpoint_loads_into_the_b200_model(tmp_path):
     """A checkpoint in the reference's format (nnUNetTrainer.py:1093-1104), with the DataParallel / torch.compile key
-    prefixes its loader tolerates (:1116-1121), loads strictly into the B200 module."""
+    prefixes its loader tolerates (:1116-1121), loads strictly into the native module."""
     import os
     import torch
     import dinounet_b200

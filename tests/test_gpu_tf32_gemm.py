@@ -1,4 +1,4 @@
-"""-m gpu: the tcgen05 kind::tf32 GEMM of the training path (csrc/gemm_tf32.cu, `b2u_tf32_gemm`) in every addressing mode
+"""-m gpu: the TF32 tensor-core GEMM of the training path (csrc/gemm_tf32.cu, `b2u_tf32_gemm`) in every addressing mode
 of its parameter block, against fp64 torch references computed on TF32-ROUNDED operands (round-to-nearest-away to 10
 mantissa bits = cvt.rna.tf32.f32, emulated bit-exactly below): what remains is fp32 accumulation order, so the
 tolerance is 2e-4 of the largest output (a misplaced chunk / swizzle / descriptor is an O(1) error).  Then the three

@@ -76,14 +76,12 @@ def test_gradients_match_the_reference_autograd_goldens():
 
 
 def test_tensor_core_tier_gradients_stay_within_tf32_of_the_goldens():
-    """The same goldens through the tcgen05 kind::tf32 matrix products (train_gemm = "tf32", the default of the train step).
+    """The same goldens through the TF32 tensor-core matrix products (train_gemm = "tf32", the default of the train step).
     Operands carry 10 mantissa bits - the fp16 autocast the reference trains under has the same - and single gradient elements
-    of this random-init network are ill-conditioned: the fp32 SIMT tier itself sits at 5.6e-4 median / 6.4e-3 worst relative
-    L2 error per tensor against fp32 autograd on the same GPU, the tf32 tier at 5.7e-2 / 1.2e-1 with a cosine of 0.9995 over
-    all gradients (tools/grad_tier_report.py -> profiles/r02_grad_tier_report.json, full tensors; the reference's own fp16
-    autocast regime overflows to NaN on these synthetic weights, as it does in the forward).  Bars at about 2x measured:
-    loss 2e-3 (1.1e-4), per-tensor norm 5e-2 (2.5e-2), and over ALL sampled elements, each tensor scaled to unit RMS, a
-    relative L2 error of 0.15 and a cosine of 0.98 (an addressing / tier mix-up is an O(1) error in these numbers)."""
+    of this random-init network are ill-conditioned (tools/grad_tier_report.py compares the tiers on full tensors; the
+    reference's own fp16 autocast regime overflows to NaN on these synthetic weights, as it does in the forward).  Bars:
+    loss 2e-3, per-tensor norm 5e-2, and over ALL sampled elements, each tensor scaled to unit RMS, a relative L2 error of
+    0.15 and a cosine of 0.98 (an addressing / tier mix-up is an O(1) error in these numbers)."""
     files = sorted(glob.glob(os.path.join(os.path.dirname(__file__), "golden", "grads_*.npz")))
     assert files
     for f in files:

@@ -4,7 +4,7 @@ csrc/gemm_tf32_addr.h holds every index computation of gemm_tf32_kernel (operand
 swizzled shared-memory offset, K slicing, epilogue placement) as host/device functions; tests/native/tf32_hostsim.cpp runs
 them for all 256 threads of every CTA and models the tensor core's read-out of the SWIZZLE_128B K-major tiles.  The test
 bodies of tests/test_gpu_tf32_gemm.py (all modes, tails, split-K, remaps) run against that model here, so what is left for
-the GPU run is the tcgen05 / mbarrier plumbing, not the arithmetic of addresses."""
+the GPU run is the wgmma plumbing, not the arithmetic of addresses."""
 import ctypes as C
 import os
 import shutil

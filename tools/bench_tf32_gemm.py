@@ -1,4 +1,4 @@
-"""Microbenchmark: the training path's matrix products on both tiers (b2u_tf32_gemm = tcgen05 kind::tf32, b2u_f32_gemm =
+"""Microbenchmark: the training path's matrix products on both tiers (b2u_tf32_gemm = TF32 wgmma, b2u_f32_gemm =
 fp32 SIMT) at the shapes that dominate the dinounet_b train step.  CUDA events, 1 warm-up + 3 timed launches each.
 usage: python tools/bench_tf32_gemm.py [B] [tiers]   (B = images for the conv shapes, default 8; tiers = "tf32,fp32")"""
 import json

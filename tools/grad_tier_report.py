@@ -1,9 +1,9 @@
-"""Conditioning report for the training path's gradient tiers (run on a B200).
+"""Conditioning report for the training path's gradient tiers (run on the GPU).
 
 For the gradient-golden case (dinounet_s, B=2, 128x128): FULL gradient tensors of
   gold  = the oracle port's autograd in fp32 on the GPU (cuDNN / cuBLAS TF32 off) - checked against the committed goldens,
   fp32  = this repo's training path, matrix products on the fp32 SIMT tier,
-  tf32  = this repo's training path, matrix products on tcgen05 kind::tf32 (the default tier),
+  tf32  = this repo's training path, matrix products on the TF32 tensor cores (the default tier),
   ref16 = the oracle port under the reference's regime (fp16 autocast, inner bf16 ViT), loss scaled by 1024,
 and per tensor  rel_l2 = |g - gold| / |gold|  and the norm error.  The point: how ill-conditioned single gradient
 elements are at random init (fp32-tier error x ~8000 = tf32-tier error), and that the tf32 tier sits at or below the
