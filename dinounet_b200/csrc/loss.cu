@@ -6,6 +6,14 @@
 // B*C*H*W.  Here ONE pass reads the logits and labels once and produces every sum (block partials in fp64, fixed
 // reduction order -> deterministic), a one-block epilogue forms the loss, and a second pass writes dLoss/dlogits.
 // HBM-bound: (4C + label) B/pixel forward, (8C + label) B/pixel backward.
+//
+// Region-based training (DC_and_BCE_loss, compound_losses.py:59-99, sigmoid Dice with do_bg, optional ignore channel)
+// uses the same three-step shape on [B, R, plane] logits and [B, R(+1), plane] real-valued targets.
+//
+// Data-parallel batch Dice (dice.py:106-110): the split entry points stop after the statistics pass with the per-class
+// batch sums [C][3] (intersect, sum_pred, sum_gt; fp64, on the device), which the caller all-reduces across ranks before
+// the finalisation.  The backward takes the incoming gradient as device scalars: the CE/BCE part is scaled by the local
+// one, the Dice part by the all-reduced one (the backward of AllGatherGrad, ddp_allgather.py:43-48).  No host sync.
 #include "common.cuh"
 #include "host_util.h"
 #include "gemm_common.h"
@@ -50,16 +58,47 @@ __device__ __forceinline__ void pixel_softmax(const float* __restrict__ z, long 
   lse = logf(s);
 }
 
+// target value as a real number (region targets are used as they are, not as booleans)
+__device__ __forceinline__ float value_at(const void* t, int kind, long long i) {
+  switch (kind) {
+    case 0: return static_cast<float>(static_cast<const uint8_t*>(t)[i]);
+    case 1: return static_cast<float>(static_cast<const int32_t*>(t)[i]);
+    case 2: return static_cast<float>(static_cast<const int64_t*>(t)[i]);
+    default: return static_cast<const float*>(t)[i];
+  }
+}
+
+// fp64 block reduction (256 threads) of N per-thread fp32 sums in a fixed order; thread k < N writes sum k to out[k]
+template <int N>
+__device__ __forceinline__ void block_sum_store(const float (&acc)[N], double* __restrict__ out) {
+  static_assert(N <= 256, "one output per thread");
+  __shared__ double red[8][N];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int k = 0; k < N; ++k) {
+    double v = static_cast<double>(acc[k]);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if (lane == 0) red[warp][k] = v;
+  }
+  __syncthreads();
+  if (threadIdx.x < N) {
+    double v = 0;
+    for (int w = 0; w < 8; ++w) v += red[w][threadIdx.x];
+    out[threadIdx.x] = v;
+  }
+}
+
 template <int C>
 __global__ void __launch_bounds__(256) loss_stats_kernel(const float* __restrict__ logits, const void* __restrict__ target,
                                                          int tkind, double* __restrict__ partial, int* __restrict__ bad,
                                                          long long plane) {
   const int b = blockIdx.y;
   const float* zb = logits + static_cast<long long>(b) * C * plane;
-  float acc[C * kStat];
-  float ce = 0.f;
+  constexpr int K = C * kStat + 1;  // the last sum is the CE
+  float acc[K];
 #pragma unroll
-  for (int k = 0; k < C * kStat; ++k) acc[k] = 0.f;
+  for (int k = 0; k < K; ++k) acc[k] = 0.f;
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < plane;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     float p[C], mx, lse;
@@ -67,7 +106,7 @@ __global__ void __launch_bounds__(256) loss_stats_kernel(const float* __restrict
     pixel_softmax<C>(zb + i, plane, p, mx, lse, amax);
     int t = label_at(target, tkind, static_cast<long long>(b) * plane + i);
     if (t < 0 || t >= C) { *bad = 1; t = 0; }
-    ce += lse - (zb[t * plane + i] - mx);
+    acc[C * kStat] += lse - (zb[t * plane + i] - mx);
 #pragma unroll
     for (int c = 0; c < C; ++c) {
       const float y = t == c ? 1.f : 0.f, h = amax == c ? 1.f : 0.f;
@@ -79,35 +118,44 @@ __global__ void __launch_bounds__(256) loss_stats_kernel(const float* __restrict
       acc[c * kStat + 5] += (1.f - h) * y;
     }
   }
-  // block reduction in fp64, fixed order
-  __shared__ double red[8][C * kStat + 1];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = 0; k <= C * kStat; ++k) {
-    double v = static_cast<double>(k < C * kStat ? acc[k < C * kStat ? k : 0] : ce);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if (lane == 0) red[warp][k] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x <= C * kStat) {
-    double v = 0;
-    for (int w = 0; w < 8; ++w) v += red[w][threadIdx.x];
-    partial[(static_cast<long long>(b) * gridDim.x + blockIdx.x) * (C * kStat + 1) + threadIdx.x] = v;
-  }
+  block_sum_store<K>(acc, partial + (static_cast<long long>(b) * gridDim.x + blockIdx.x) * K);
 }
 
-// stats: double [B][C*6 + 1] (the +1 is the sample's CE sum).  out: float[3] = loss, ce, dice term.
-__global__ void loss_finalize_kernel(const double* __restrict__ partial, double* __restrict__ stats,
-                                     float* __restrict__ out, int64_t* __restrict__ tpfpfn, int B, int C, int nblk,
-                                     long long plane, float w_ce, float w_dice, int batch_dice, int do_bg, float smooth) {
-  const int K = C * kStat + 1;
+// stats[b][k] = sum over the blocks of sample b of partial sum k, in block order
+__device__ __forceinline__ void reduce_sample_stats(const double* __restrict__ partial, double* __restrict__ stats, int B,
+                                                    int K, int nblk) {
   for (int j = threadIdx.x; j < B * K; j += blockDim.x) {
     const int b = j / K, k = j - b * K;
     double v = 0;
     for (int n = 0; n < nblk; ++n) v += partial[(static_cast<long long>(b) * nblk + n) * K + k];
     stats[j] = v;
   }
+}
+
+// bsum[c][3] = (intersect, sum_pred, sum_gt) of class c over the batch: per sample in block order, then in sample
+// order, which is the order the fused finalisation sums in.  K = per-sample record length; class c's record at c*kStat.
+__global__ void dice_batch_sums_kernel(const double* __restrict__ partial, double* __restrict__ bsum, int B, int C,
+                                       int K, int nblk) {
+  for (int j = threadIdx.x; j < C * 3; j += blockDim.x) {
+    const int c = j / 3, s = j - c * 3;
+    double v = 0;
+    for (int b = 0; b < B; ++b) {
+      double vb = 0;
+      for (int n = 0; n < nblk; ++n) vb += partial[(static_cast<long long>(b) * nblk + n) * K + c * kStat + s];
+      v += vb;
+    }
+    bsum[j] = v;
+  }
+}
+
+// stats: double [B][C*6 + 1] (the +1 is the sample's CE sum).  out: float[3] = loss, ce, dice term.
+// gsum (optional): batch sums [C][3] to take the batch Dice from (all-reduced across data-parallel ranks).
+__global__ void loss_finalize_kernel(const double* __restrict__ partial, double* __restrict__ stats,
+                                     const double* __restrict__ gsum, float* __restrict__ out,
+                                     int64_t* __restrict__ tpfpfn, int B, int C, int nblk, long long plane, float w_ce,
+                                     float w_dice, int batch_dice, int do_bg, float smooth) {
+  const int K = C * kStat + 1;
+  reduce_sample_stats(partial, stats, B, K, nblk);
   __syncthreads();
   if (threadIdx.x != 0) return;
   double ce = 0;
@@ -118,10 +166,16 @@ __global__ void loss_finalize_kernel(const double* __restrict__ partial, double*
   if (batch_dice) {
     for (int c = c0; c < C; ++c) {
       double I = 0, P = 0, G = 0;
-      for (int b = 0; b < B; ++b) {
-        I += stats[b * K + c * kStat];
-        P += stats[b * K + c * kStat + 1];
-        G += stats[b * K + c * kStat + 2];
+      if (gsum) {
+        I = gsum[c * 3];
+        P = gsum[c * 3 + 1];
+        G = gsum[c * 3 + 2];
+      } else {
+        for (int b = 0; b < B; ++b) {
+          I += stats[b * K + c * kStat];
+          P += stats[b * K + c * kStat + 1];
+          G += stats[b * K + c * kStat + 2];
+        }
       }
       dc += (2 * I + smooth) / fmax(G + P + smooth, 1e-8);
     }
@@ -149,9 +203,11 @@ __global__ void loss_finalize_kernel(const double* __restrict__ partial, double*
 template <int C>
 __global__ void __launch_bounds__(256) loss_grad_kernel(const float* __restrict__ logits, const void* __restrict__ target,
                                                         int tkind, const double* __restrict__ stats,
-                                                        float* __restrict__ grad, int B, long long plane, float w_ce,
-                                                        float w_dice, int batch_dice, int do_bg, float smooth,
-                                                        float grad_scale) {
+                                                        const double* __restrict__ gsum, float* __restrict__ grad,
+                                                        int B, long long plane, float w_ce, float w_dice, int batch_dice,
+                                                        int do_bg, float smooth, float grad_scale,
+                                                        const float* __restrict__ ce_scale,
+                                                        const float* __restrict__ dice_scale) {
   const int b = blockIdx.y;
   constexpr int K = C * kStat + 1;
   // per-class dice coefficients a_c, b_c with d(dice term)/dp_c = a_c * y_c + b_c
@@ -161,23 +217,30 @@ __global__ void __launch_bounds__(256) loss_grad_kernel(const float* __restrict_
     float a = 0.f, bb = 0.f;
     if (c >= c0) {
       double I = 0, P = 0, G = 0;
-      for (int n = batch_dice ? 0 : b; n < (batch_dice ? B : b + 1); ++n) {
-        I += stats[n * K + c * kStat];
-        P += stats[n * K + c * kStat + 1];
-        G += stats[n * K + c * kStat + 2];
+      if (batch_dice && gsum) {
+        I = gsum[c * 3];
+        P = gsum[c * 3 + 1];
+        G = gsum[c * 3 + 2];
+      } else {
+        for (int n = batch_dice ? 0 : b; n < (batch_dice ? B : b + 1); ++n) {
+          I += stats[n * K + c * kStat];
+          P += stats[n * K + c * kStat + 1];
+          G += stats[n * K + c * kStat + 2];
+        }
       }
       const double num = 2 * I + smooth, raw = G + P + smooth, den = fmax(raw, 1e-8);
       const double cnt = batch_dice ? static_cast<double>(C - c0) : static_cast<double>(B) * (C - c0);
       a = static_cast<float>(-2.0 / (den * cnt));                              // through the intersection
       bb = raw > 1e-8 ? static_cast<float>(num / (den * den * cnt)) : 0.f;      // through sum_pred (clip passes no grad)
     }
-    sa[c] = a;
-    sb[c] = bb;
+    const float ds = dice_scale ? *dice_scale : 1.f;
+    sa[c] = a * ds;
+    sb[c] = bb * ds;
   }
   __syncthreads();
   const float* zb = logits + static_cast<long long>(b) * C * plane;
   float* gb = grad + static_cast<long long>(b) * C * plane;
-  const float ce_w = w_ce / (static_cast<float>(B) * static_cast<float>(plane));
+  const float ce_w = w_ce / (static_cast<float>(B) * static_cast<float>(plane)) * (ce_scale ? *ce_scale : 1.f);
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < plane;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     float p[C], mx, lse;
@@ -197,12 +260,165 @@ __global__ void __launch_bounds__(256) loss_grad_kernel(const float* __restrict_
   }
 }
 
+// ---- region-based (sigmoid) Dice + BCE.  Per (sample, region): intersect, sum_pred, sum_gt over valid pixels and the
+// validation tp, fp, fn of sigmoid(z) > 0.5 weighted by 1 - t_ign; per sample: BCE sum over valid pixels, valid count.
+constexpr int kRegionExtra = 2;
+
+__device__ __forceinline__ float bce_with_logits(float z, float y) {
+  return fmaxf(z, 0.f) - z * y + log1pf(expf(-fabsf(z)));
+}
+
+template <int R>
+__global__ void __launch_bounds__(256) region_stats_kernel(const float* __restrict__ logits, const void* __restrict__ target,
+                                                           int tkind, int has_ignore, double* __restrict__ partial,
+                                                           long long plane) {
+  const int b = blockIdx.y;
+  const float* zb = logits + static_cast<long long>(b) * R * plane;
+  const long long tb = static_cast<long long>(b) * (R + has_ignore) * plane;
+  constexpr int K = R * kStat + kRegionExtra;
+  float acc[K];
+#pragma unroll
+  for (int k = 0; k < K; ++k) acc[k] = 0.f;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < plane;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    float w = 1.f, m = 1.f;  // validation weight 1 - t_ign, loss mask (1 - t_ign) != 0
+    if (has_ignore) {
+      w = 1.f - value_at(target, tkind, tb + R * plane + i);
+      m = w != 0.f ? 1.f : 0.f;
+    }
+    float bce = 0.f;
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      const float z = zb[r * plane + i], y = value_at(target, tkind, tb + r * plane + i);
+      const float x = 1.f / (1.f + expf(-z));
+      const float h = x > 0.5f ? 1.f : 0.f;  // == torch.sigmoid(z) > 0.5 on fp32 (fast math is off)
+      acc[r * kStat + 0] += x * y * m;
+      acc[r * kStat + 1] += x * m;
+      acc[r * kStat + 2] += y * m;
+      acc[r * kStat + 3] += h * y * w;
+      acc[r * kStat + 4] += h * (1.f - y) * w;
+      acc[r * kStat + 5] += (1.f - h) * y * w;
+      bce += bce_with_logits(z, y);
+    }
+    acc[R * kStat] += bce * m;
+    acc[R * kStat + 1] += m;
+  }
+  block_sum_store<K>(acc, partial + (static_cast<long long>(b) * gridDim.x + blockIdx.x) * K);
+}
+
+// out: float[3] = loss, BCE, dice term.  tpfpfn: float [3][R] summed over the batch.
+__global__ void region_finalize_kernel(const double* __restrict__ partial, double* __restrict__ stats,
+                                       const double* __restrict__ bsum, float* __restrict__ out,
+                                       float* __restrict__ tpfpfn, int B, int R, int nblk, long long plane, float w_ce,
+                                       float w_dice, int batch_dice, int has_ignore, float smooth) {
+  const int K = R * kStat + kRegionExtra;
+  reduce_sample_stats(partial, stats, B, K, nblk);
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  double bce = 0, valid = 0;
+  for (int b = 0; b < B; ++b) {
+    bce += stats[b * K + R * kStat];
+    valid += stats[b * K + R * kStat + 1];
+  }
+  // masked: sum(bce * mask) / clip(#valid pixels, 1e-8) -- pixels, not pixel x region pairs (compound_losses.py:95)
+  bce /= has_ignore ? fmax(valid, 1e-8) : static_cast<double>(B) * R * static_cast<double>(plane);
+  double dc = 0;
+  if (batch_dice) {
+    for (int r = 0; r < R; ++r)
+      dc += (2 * bsum[r * 3] + smooth) / fmax(bsum[r * 3 + 2] + bsum[r * 3 + 1] + smooth, 1e-8);
+    dc /= R;
+  } else {
+    for (int b = 0; b < B; ++b)
+      for (int r = 0; r < R; ++r) {
+        const double I = stats[b * K + r * kStat], P = stats[b * K + r * kStat + 1], G = stats[b * K + r * kStat + 2];
+        dc += (2 * I + smooth) / fmax(G + P + smooth, 1e-8);
+      }
+    dc /= static_cast<double>(B) * R;
+  }
+  out[1] = static_cast<float>(bce);
+  out[2] = static_cast<float>(-dc);
+  out[0] = static_cast<float>(w_ce * bce - w_dice * dc);
+  if (tpfpfn)
+    for (int r = 0; r < R; ++r)
+      for (int s = 0; s < 3; ++s) {
+        double v = 0;
+        for (int b = 0; b < B; ++b) v += stats[b * K + r * kStat + 3 + s];
+        tpfpfn[s * R + r] = static_cast<float>(v);
+      }
+}
+
+template <int R>
+__global__ void __launch_bounds__(256) region_grad_kernel(const float* __restrict__ logits, const void* __restrict__ target,
+                                                          int tkind, int has_ignore, const double* __restrict__ stats,
+                                                          const double* __restrict__ bsum, float* __restrict__ grad,
+                                                          int B, long long plane, float w_ce, float w_dice,
+                                                          int batch_dice, float smooth,
+                                                          const float* __restrict__ ce_scale,
+                                                          const float* __restrict__ dice_scale) {
+  const int b = blockIdx.y;
+  constexpr int K = R * kStat + kRegionExtra;
+  // d(dice term)/dx_r = (a_r * y_r + b_r) * m;  d BCE / dz_r = bce_w * (x_r - y_r) * m
+  __shared__ float sa[R], sb[R], s_bce;
+  if (threadIdx.x < R) {
+    const int r = threadIdx.x;
+    double I = 0, P = 0, G = 0;
+    if (batch_dice) {
+      I = bsum[r * 3];
+      P = bsum[r * 3 + 1];
+      G = bsum[r * 3 + 2];
+    } else {
+      I = stats[b * K + r * kStat];
+      P = stats[b * K + r * kStat + 1];
+      G = stats[b * K + r * kStat + 2];
+    }
+    const double num = 2 * I + smooth, raw = G + P + smooth, den = fmax(raw, 1e-8);
+    const double cnt = batch_dice ? static_cast<double>(R) : static_cast<double>(B) * R;
+    const float ds = w_dice * (dice_scale ? *dice_scale : 1.f);
+    sa[r] = ds * static_cast<float>(-2.0 / (den * cnt));
+    sb[r] = raw > 1e-8 ? ds * static_cast<float>(num / (den * den * cnt)) : 0.f;  // the clip passes no gradient
+  }
+  if (threadIdx.x == 32) {
+    double norm = static_cast<double>(B) * R * static_cast<double>(plane);
+    if (has_ignore) {
+      double valid = 0;
+      for (int n = 0; n < B; ++n) valid += stats[n * K + R * kStat + 1];
+      norm = fmax(valid, 1e-8);
+    }
+    s_bce = static_cast<float>(w_ce / norm) * (ce_scale ? *ce_scale : 1.f);
+  }
+  __syncthreads();
+  const float* zb = logits + static_cast<long long>(b) * R * plane;
+  float* gb = grad + static_cast<long long>(b) * R * plane;
+  const long long tb = static_cast<long long>(b) * (R + has_ignore) * plane;
+  const float bw = s_bce;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < plane;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    float m = 1.f;
+    if (has_ignore) m = 1.f - value_at(target, tkind, tb + R * plane + i) != 0.f ? 1.f : 0.f;
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      const float z = zb[r * plane + i], y = value_at(target, tkind, tb + r * plane + i);
+      const float x = 1.f / (1.f + expf(-z));
+      gb[r * plane + i] = m * (bw * (x - y) + x * (1.f - x) * (sa[r] * y + sb[r]));
+    }
+  }
+}
+
 static int stats_blocks(long long plane) {
   return static_cast<int>(std::max<long long>(1, std::min<long long>((plane + 256 * 16 - 1) / (256 * 16), 1024)));
 }
 
+static int grad_blocks(long long plane) {
+  return static_cast<int>(std::max<long long>(1, std::min<long long>((plane + 1023) / 1024, 4096)));
+}
+
 extern "C" int64_t b2u_dice_ce_work_doubles(int32_t B, int32_t C, int64_t plane) {
   return static_cast<int64_t>(B) * stats_blocks(plane) * (C * kStat + 1) + static_cast<int64_t>(B) * (C * kStat + 1);
+}
+
+extern "C" int64_t b2u_dice_bce_work_doubles(int32_t B, int32_t R, int64_t plane) {
+  const int64_t K = R * kStat + kRegionExtra;
+  return static_cast<int64_t>(B) * stats_blocks(plane) * K + static_cast<int64_t>(B) * K;
 }
 
 // one instantiation per class count: every per-class sum lives in a named register (large counts spill, which is fine
@@ -243,6 +459,24 @@ extern "C" int64_t b2u_dice_ce_work_doubles(int32_t B, int32_t C, int64_t plane)
     default: return set_error(-1, "dice_ce: %d classes not in [2, 32]", C);                    \
   }
 
+// regions: one instantiation per region count, 1 <= R <= 32 (a single region is one sigmoid head)
+#define B2U_REGION_SWITCH(R, BODY)    \
+  if ((R) == 1) {                     \
+    constexpr int CC = 1;             \
+    BODY                              \
+  } else {                            \
+    B2U_LOSS_SWITCH(R, BODY)          \
+  }
+
+static int dice_ce_stats(const float* logits, const void* target, int32_t target_kind, double* work,
+                         int32_t* bad_label, int32_t B, int32_t C, int64_t plane, cudaStream_t stream) {
+  const int nblk = stats_blocks(plane);
+  dim3 grid(nblk, B);
+  B2U_LOSS_SWITCH(C, (loss_stats_kernel<CC><<<grid, 256, 0, stream>>>(logits, target, target_kind, work, bad_label,
+                                                                      plane));)
+  return check_launch("dice_ce_stats");
+}
+
 extern "C" int b2u_dice_ce_forward(const float* logits, const void* target, int32_t target_kind, double* work,
                                    float* out3, int64_t* tp_fp_fn, int32_t* bad_label, int32_t B, int32_t C,
                                    int64_t plane, float weight_ce, float weight_dice, int32_t batch_dice, int32_t do_bg,
@@ -251,33 +485,125 @@ extern "C" int b2u_dice_ce_forward(const float* logits, const void* target, int3
   if (!logits || !target || !work || !out3 || !bad_label) return set_error(-1, "b2u_dice_ce_forward: null pointer");
   if (B <= 0 || plane <= 0 || target_kind < 0 || target_kind > 3) return set_error(-1, "b2u_dice_ce_forward: bad argument");
   if (!do_bg && C < 2) return set_error(-1, "b2u_dice_ce_forward: do_bg=0 needs >= 2 classes");
+  if (int rc = dice_ce_stats(logits, target, target_kind, work, bad_label, B, C, plane, stream)) return rc;
   const int nblk = stats_blocks(plane);
-  double* partial = work;
   double* stats = work + static_cast<int64_t>(B) * nblk * (C * kStat + 1);
-  dim3 grid(nblk, B);
-  B2U_LOSS_SWITCH(C, (loss_stats_kernel<CC><<<grid, 256, 0, stream>>>(logits, target, target_kind, partial, bad_label,
-                                                                      plane));)
-  if (int rc = check_launch("dice_ce_stats")) return rc;
-  loss_finalize_kernel<<<1, 256, 0, stream>>>(partial, stats, out3, tp_fp_fn, B, C, nblk, plane, weight_ce, weight_dice,
-                                              batch_dice, do_bg, smooth);
+  loss_finalize_kernel<<<1, 256, 0, stream>>>(work, stats, nullptr, out3, tp_fp_fn, B, C, nblk, plane, weight_ce,
+                                              weight_dice, batch_dice, do_bg, smooth);
   return check_launch("dice_ce_finalize");
+}
+
+extern "C" int b2u_dice_ce_stats(const float* logits, const void* target, int32_t target_kind, double* work,
+                                 double* batch_sums, int32_t* bad_label, int32_t B, int32_t C, int64_t plane,
+                                 b2u_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (!logits || !target || !work || !batch_sums || !bad_label) return set_error(-1, "b2u_dice_ce_stats: null pointer");
+  if (B <= 0 || plane <= 0 || target_kind < 0 || target_kind > 3) return set_error(-1, "b2u_dice_ce_stats: bad argument");
+  if (int rc = dice_ce_stats(logits, target, target_kind, work, bad_label, B, C, plane, stream)) return rc;
+  dice_batch_sums_kernel<<<1, 128, 0, stream>>>(work, batch_sums, B, C, C * kStat + 1, stats_blocks(plane));
+  return check_launch("dice_ce_batch_sums");
+}
+
+extern "C" int b2u_dice_ce_finalize(double* work, const double* batch_sums, float* out3, int64_t* tp_fp_fn, int32_t B,
+                                    int32_t C, int64_t plane, float weight_ce, float weight_dice, int32_t batch_dice,
+                                    int32_t do_bg, float smooth, b2u_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (!work || !batch_sums || !out3) return set_error(-1, "b2u_dice_ce_finalize: null pointer");
+  if (B <= 0 || plane <= 0 || C < 2 || C > 32) return set_error(-1, "b2u_dice_ce_finalize: bad argument");
+  const int nblk = stats_blocks(plane);
+  double* stats = work + static_cast<int64_t>(B) * nblk * (C * kStat + 1);
+  loss_finalize_kernel<<<1, 256, 0, stream>>>(work, stats, batch_sums, out3, tp_fp_fn, B, C, nblk, plane, weight_ce,
+                                              weight_dice, batch_dice, do_bg, smooth);
+  return check_launch("dice_ce_finalize");
+}
+
+static int dice_ce_grad(const float* logits, const void* target, int32_t target_kind, const double* work,
+                        const double* batch_sums, float* grad_logits, int32_t B, int32_t C, int64_t plane,
+                        float weight_ce, float weight_dice, int32_t batch_dice, int32_t do_bg, float smooth,
+                        float grad_scale, const float* ce_scale, const float* dice_scale, cudaStream_t stream) {
+  if (!logits || !target || !work || !grad_logits) return set_error(-1, "b2u_dice_ce_backward: null pointer");
+  if (target_kind < 0 || target_kind > 3) return set_error(-1, "b2u_dice_ce_backward: bad target kind");
+  const int nblk = stats_blocks(plane);
+  const double* stats = work + static_cast<int64_t>(B) * nblk * (C * kStat + 1);
+  dim3 grid(grad_blocks(plane), B);
+  B2U_LOSS_SWITCH(C, (loss_grad_kernel<CC><<<grid, 256, 0, stream>>>(logits, target, target_kind, stats, batch_sums,
+                                                                     grad_logits, B, plane, weight_ce, weight_dice,
+                                                                     batch_dice, do_bg, smooth, grad_scale, ce_scale,
+                                                                     dice_scale));)
+  return check_launch("dice_ce_backward");
 }
 
 extern "C" int b2u_dice_ce_backward(const float* logits, const void* target, int32_t target_kind, const double* work,
                                     float* grad_logits, int32_t B, int32_t C, int64_t plane, float weight_ce,
                                     float weight_dice, int32_t batch_dice, int32_t do_bg, float smooth,
                                     float grad_scale, b2u_stream_t stream_) {
+  return dice_ce_grad(logits, target, target_kind, work, nullptr, grad_logits, B, C, plane, weight_ce, weight_dice,
+                      batch_dice, do_bg, smooth, grad_scale, nullptr, nullptr, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int b2u_dice_ce_backward_scaled(const float* logits, const void* target, int32_t target_kind,
+                                           const double* work, const double* batch_sums, float* grad_logits, int32_t B,
+                                           int32_t C, int64_t plane, float weight_ce, float weight_dice,
+                                           int32_t batch_dice, int32_t do_bg, float smooth, const float* ce_scale,
+                                           const float* dice_scale, b2u_stream_t stream_) {
+  if (!batch_sums || !ce_scale || !dice_scale) return set_error(-1, "b2u_dice_ce_backward_scaled: null pointer");
+  return dice_ce_grad(logits, target, target_kind, work, batch_sums, grad_logits, B, C, plane, weight_ce, weight_dice,
+                      batch_dice, do_bg, smooth, 1.f, ce_scale, dice_scale, static_cast<cudaStream_t>(stream_));
+}
+
+static int region_args(const char* fn, const float* logits, const void* target, int32_t target_kind, int32_t B,
+                       int32_t R, int64_t plane) {
+  if (!logits || !target) return set_error(-1, "%s: null pointer", fn);
+  if (B <= 0 || plane <= 0 || target_kind < 0 || target_kind > 3) return set_error(-1, "%s: bad argument", fn);
+  if (R < 1 || R > 32) return set_error(-1, "%s: %d regions not in [1, 32]", fn, R);
+  return 0;
+}
+
+extern "C" int b2u_dice_bce_stats(const float* logits, const void* target, int32_t target_kind, int32_t has_ignore,
+                                  double* work, double* batch_sums, int32_t B, int32_t R, int64_t plane,
+                                  b2u_stream_t stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (!logits || !target || !work || !grad_logits) return set_error(-1, "b2u_dice_ce_backward: null pointer");
-  if (target_kind < 0 || target_kind > 3) return set_error(-1, "b2u_dice_ce_backward: bad target kind");
+  if (int rc = region_args("b2u_dice_bce_stats", logits, target, target_kind, B, R, plane)) return rc;
+  if (!work || !batch_sums) return set_error(-1, "b2u_dice_bce_stats: null pointer");
+  const int nblk = stats_blocks(plane), ign = has_ignore ? 1 : 0;
+  dim3 grid(nblk, B);
+  B2U_REGION_SWITCH(R, (region_stats_kernel<CC><<<grid, 256, 0, stream>>>(logits, target, target_kind, ign, work,
+                                                                          plane));)
+  if (int rc = check_launch("dice_bce_stats")) return rc;
+  dice_batch_sums_kernel<<<1, 128, 0, stream>>>(work, batch_sums, B, R, R * kStat + kRegionExtra, nblk);
+  return check_launch("dice_bce_batch_sums");
+}
+
+extern "C" int b2u_dice_bce_finalize(double* work, const double* batch_sums, float* out3, float* tp_fp_fn, int32_t B,
+                                     int32_t R, int64_t plane, float weight_ce, float weight_dice, int32_t batch_dice,
+                                     int32_t has_ignore, float smooth, b2u_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (!work || !batch_sums || !out3) return set_error(-1, "b2u_dice_bce_finalize: null pointer");
+  if (B <= 0 || plane <= 0 || R < 1 || R > 32) return set_error(-1, "b2u_dice_bce_finalize: bad argument");
   const int nblk = stats_blocks(plane);
-  const double* stats = work + static_cast<int64_t>(B) * nblk * (C * kStat + 1);
-  const int gblk = static_cast<int>(std::max<long long>(1, std::min<long long>((plane + 1023) / 1024, 4096)));
-  dim3 grid(gblk, B);
-  B2U_LOSS_SWITCH(C, (loss_grad_kernel<CC><<<grid, 256, 0, stream>>>(logits, target, target_kind, stats, grad_logits, B,
-                                                                     plane, weight_ce, weight_dice, batch_dice, do_bg,
-                                                                     smooth, grad_scale));)
-  return check_launch("dice_ce_backward");
+  double* stats = work + static_cast<int64_t>(B) * nblk * (R * kStat + kRegionExtra);
+  region_finalize_kernel<<<1, 256, 0, stream>>>(work, stats, batch_sums, out3, tp_fp_fn, B, R, nblk, plane, weight_ce,
+                                                weight_dice, batch_dice, has_ignore ? 1 : 0, smooth);
+  return check_launch("dice_bce_finalize");
+}
+
+extern "C" int b2u_dice_bce_backward(const float* logits, const void* target, int32_t target_kind, int32_t has_ignore,
+                                     const double* work, const double* batch_sums, float* grad_logits, int32_t B,
+                                     int32_t R, int64_t plane, float weight_ce, float weight_dice, int32_t batch_dice,
+                                     float smooth, const float* ce_scale, const float* dice_scale,
+                                     b2u_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (int rc = region_args("b2u_dice_bce_backward", logits, target, target_kind, B, R, plane)) return rc;
+  if (!work || !batch_sums || !grad_logits || !ce_scale || !dice_scale)
+    return set_error(-1, "b2u_dice_bce_backward: null pointer");
+  const int nblk = stats_blocks(plane), ign = has_ignore ? 1 : 0;
+  const double* stats = work + static_cast<int64_t>(B) * nblk * (R * kStat + kRegionExtra);
+  dim3 grid(grad_blocks(plane), B);
+  B2U_REGION_SWITCH(R, (region_grad_kernel<CC><<<grid, 256, 0, stream>>>(logits, target, target_kind, ign, stats,
+                                                                         batch_sums, grad_logits, B, plane, weight_ce,
+                                                                         weight_dice, batch_dice, smooth, ce_scale,
+                                                                         dice_scale));)
+  return check_launch("dice_bce_backward");
 }
 
 }  // namespace b2u

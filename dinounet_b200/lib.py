@@ -97,6 +97,13 @@ SIGNATURES = {
     "b2u_dice_ce_work_doubles": [i32, i32, i64],
     "b2u_dice_ce_forward": [vp, vp, i32, vp, vp, vp, vp, i32, i32, i64, f32, f32, i32, i32, f32, vp],
     "b2u_dice_ce_backward": [vp, vp, i32, vp, vp, i32, i32, i64, f32, f32, i32, i32, f32, f32, vp],
+    "b2u_dice_ce_stats": [vp, vp, i32, vp, vp, vp, i32, i32, i64, vp],
+    "b2u_dice_ce_finalize": [vp, vp, vp, vp, i32, i32, i64, f32, f32, i32, i32, f32, vp],
+    "b2u_dice_ce_backward_scaled": [vp, vp, i32, vp, vp, vp, i32, i32, i64, f32, f32, i32, i32, f32, vp, vp, vp],
+    "b2u_dice_bce_work_doubles": [i32, i32, i64],
+    "b2u_dice_bce_stats": [vp, vp, i32, i32, vp, vp, i32, i32, i64, vp],
+    "b2u_dice_bce_finalize": [vp, vp, vp, vp, i32, i32, i64, f32, f32, i32, i32, f32, vp],
+    "b2u_dice_bce_backward": [vp, vp, i32, i32, vp, vp, vp, i32, i32, i64, f32, f32, i32, f32, vp, vp, vp],
     "b2u_msda_backward_f32": [vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp],
     "b2u_tail_fuse": [vp, i32, i64, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp],
     "b2u_in_stats_work_floats": [i32, i32, i32],
@@ -146,7 +153,7 @@ SIGNATURES = {
     "b2u_launch_count": [],
 }
 _RESTYPES = {"b2u_last_error": C.c_char_p, "b2u_launch_count": C.c_int64, "b2u_in_stats_work_floats": C.c_int64,
-             "b2u_dice_ce_work_doubles": C.c_int64}
+             "b2u_dice_ce_work_doubles": C.c_int64, "b2u_dice_bce_work_doubles": C.c_int64}
 
 _lib: Optional[C.CDLL] = None
 

@@ -12,7 +12,7 @@ import torch
 from torch import nn
 
 from . import config as cfg
-from .loss import DC_and_CE_loss, validation_statistics
+from .loss import DC_and_BCE_loss, DC_and_CE_loss, validation_statistics
 from .network_architecture import DinoUNet
 
 try:  # the reference package (needs batchgenerators etc.); optional
@@ -57,10 +57,14 @@ class DinoUNetTrainer(_Base):
 
     # ---- forward-only callers of the path that the trainer owns (nnUNetTrainer.py:355-365, :945-1005)
     def _build_loss(self):
-        """Label-map training: Dice (batch_dice from the plans, smooth 1e-5, no background) + CE, weights 1:1 — the
-        fused native loss.  No deep-supervision wrapper (the trainer derives from nnUNetTrainerNoDeepSupervision)."""
+        """The fused native losses with the reference's arguments.  Region-based datasets: sigmoid Dice (batch_dice from
+        the plans, every region, smooth 1e-5) + BCE, ignore channel when the dataset has an ignore label.  Label maps:
+        Dice (no background) + CE, weights 1:1.  `ddp` follows the trainer, so under DDP the batch Dice sums are taken
+        over every rank.  No deep-supervision wrapper (the trainer derives from nnUNetTrainerNoDeepSupervision)."""
         if self.label_manager.has_regions:
-            raise NotImplementedError("region-based (sigmoid/BCE) training is not covered by the fused native loss")
+            return DC_and_BCE_loss({}, {"batch_dice": self.configuration_manager.batch_dice, "do_bg": True,
+                                        "smooth": 1e-5, "ddp": self.is_ddp},
+                                   use_ignore_label=self.label_manager.ignore_label is not None)
         return DC_and_CE_loss({"batch_dice": self.configuration_manager.batch_dice, "smooth": 1e-5, "do_bg": False,
                                "ddp": self.is_ddp}, {}, weight_ce=1, weight_dice=1,
                               ignore_label=self.label_manager.ignore_label)
@@ -90,7 +94,8 @@ class DinoUNetTrainer(_Base):
         return {"loss": loss.cpu().numpy()}
 
     def validation_step(self, batch: dict) -> dict:
-        """One online-validation batch: native forward, then loss + hard tp/fp/fn in one fused pass over the logits."""
+        """One online-validation batch: native forward, then loss + hard tp/fp/fn in one fused pass over the logits
+        (argmax per class for label maps, sigmoid > 0.5 per region with the ignore channel as a weight for regions)."""
         data = batch["data"].to(self.device, non_blocking=True)
         target = batch["target"]
         if isinstance(target, list):

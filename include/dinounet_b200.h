@@ -218,7 +218,14 @@ int b2u_sw_finalize(void* acc, const void* npred, int32_t C, int64_t plane, int3
  *   batch (get_tp_fp_fn_tn with axes (0,2,3), nnUNetTrainer.py:971-991);  *bad_label is set to 1 if a label is outside
  *   [0, C) (torch raises a device assert there).  Deterministic (fixed reduction order, fp64 partials).
  * backward: grad_logits fp32 [B, C, plane] = grad_scale * dLoss/dlogits, from the sums the forward left in `work`.
- * 2 <= C <= 32.  ignore_label / region (BCE) training are not covered. */
+ * 2 <= C <= 32.  ignore_label is not covered.
+ *
+ * Split forward for data-parallel batch Dice (dice.py:106-110, AllGatherGrad): b2u_dice_ce_stats runs the statistics
+ * pass and writes batch_sums fp64 [C][3] = (intersect, sum_pred, sum_gt) of every class summed over the local batch;
+ * the caller may all-reduce batch_sums across ranks; b2u_dice_ce_finalize then forms out3 / tp_fp_fn as the fused
+ * forward does, with the batch Dice taken from batch_sums (batch_dice = 0 ignores them: per-sample Dice stays local).
+ * b2u_dice_ce_backward_scaled: grad = *ce_scale * dCE/dlogits + *dice_scale * d(dice term)/dlogits (device scalars: the
+ * local incoming gradient and its sum over ranks), Dice coefficients from batch_sums. */
 int64_t b2u_dice_ce_work_doubles(int32_t B, int32_t C, int64_t plane);
 int b2u_dice_ce_forward(const float* logits, const void* target, int32_t target_kind, double* work, float* out3,
                         int64_t* tp_fp_fn, int32_t* bad_label, int32_t B, int32_t C, int64_t plane, float weight_ce,
@@ -226,6 +233,37 @@ int b2u_dice_ce_forward(const float* logits, const void* target, int32_t target_
 int b2u_dice_ce_backward(const float* logits, const void* target, int32_t target_kind, const double* work,
                          float* grad_logits, int32_t B, int32_t C, int64_t plane, float weight_ce, float weight_dice,
                          int32_t batch_dice, int32_t do_bg, float smooth, float grad_scale, b2u_stream_t stream);
+int b2u_dice_ce_stats(const float* logits, const void* target, int32_t target_kind, double* work, double* batch_sums,
+                      int32_t* bad_label, int32_t B, int32_t C, int64_t plane, b2u_stream_t stream);
+int b2u_dice_ce_finalize(double* work, const double* batch_sums, float* out3, int64_t* tp_fp_fn, int32_t B, int32_t C,
+                         int64_t plane, float weight_ce, float weight_dice, int32_t batch_dice, int32_t do_bg,
+                         float smooth, b2u_stream_t stream);
+int b2u_dice_ce_backward_scaled(const float* logits, const void* target, int32_t target_kind, const double* work,
+                                const double* batch_sums, float* grad_logits, int32_t B, int32_t C, int64_t plane,
+                                float weight_ce, float weight_dice, int32_t batch_dice, int32_t do_bg, float smooth,
+                                const float* ce_scale, const float* dice_scale, b2u_stream_t stream);
+
+/* ---- Region-based Dice + BCE (compound_losses.py:59-99 `DC_and_BCE_loss` with MemoryEfficientSoftDiceLoss on
+ * sigmoid(logits), do_bg, built at nnUNetTrainer.py:356-361; validation_step's region branch :973-994).
+ * logits fp32 [B, R, plane], 1 <= R <= 32; target [B, R + has_ignore, plane] of target_kind (as above), used as real
+ * values; with has_ignore the last channel is the ignore channel: a pixel is valid where (1 - t_ign) != 0.
+ * work: b2u_dice_bce_work_doubles(B, R, plane) doubles.  Same split as the softmax loss:
+ * stats: one pass; batch_sums fp64 [R][3] = (intersect, sum_pred, sum_gt) over valid pixels, summed over the batch.
+ * finalize: out3[0] = weight_ce*BCE + weight_dice*dice, out3[1] = BCE (mean over B*R*plane; with has_ignore
+ *   sum(bce * valid) / max(#valid pixels, 1e-8)), out3[2] = -mean_r (2I+smooth)/max(G+P+smooth, 1e-8) (batch Dice from
+ *   batch_sums, else per sample);  tp_fp_fn (optional) float [3][R] = sum over the batch of pred*y*w, pred*(1-y)*w,
+ *   (1-pred)*y*w with pred = sigmoid(z) > 0.5 and w = 1 - t_ign (1 without an ignore channel).
+ * backward: grad = *ce_scale * dBCE/dlogits + *dice_scale * d(dice term)/dlogits.  Deterministic. */
+int64_t b2u_dice_bce_work_doubles(int32_t B, int32_t R, int64_t plane);
+int b2u_dice_bce_stats(const float* logits, const void* target, int32_t target_kind, int32_t has_ignore, double* work,
+                       double* batch_sums, int32_t B, int32_t R, int64_t plane, b2u_stream_t stream);
+int b2u_dice_bce_finalize(double* work, const double* batch_sums, float* out3, float* tp_fp_fn, int32_t B, int32_t R,
+                          int64_t plane, float weight_ce, float weight_dice, int32_t batch_dice, int32_t has_ignore,
+                          float smooth, b2u_stream_t stream);
+int b2u_dice_bce_backward(const float* logits, const void* target, int32_t target_kind, int32_t has_ignore,
+                          const double* work, const double* batch_sums, float* grad_logits, int32_t B, int32_t R,
+                          int64_t plane, float weight_ce, float weight_dice, int32_t batch_dice, float smooth,
+                          const float* ce_scale, const float* dice_scale, b2u_stream_t stream);
 
 /* Adapter tail (dinov3_adapter.py:467-482): out[b,y,x,:] = BN_eval( base[b,y,x,:] + bilinear(tap[b,:,:,:] -> HxW) ).
  * base: fp32 token stream slice or 16-bit image (base_fp32), tap fp32 [B, Ht*Wt, D] (token-major), align_corners=False. */
