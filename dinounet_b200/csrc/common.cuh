@@ -48,6 +48,14 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
 // blocks of the next kernel sit on the SMs next to the running one; the implicit trigger at block exit is kept instead.)
 __device__ __forceinline__ void pdl_begin() { pdl_wait(); }
 
+// ---------------------------------------------------------------- per-warpgroup register budget (sm_90a setmaxnreg)
+// Every warp of the warpgroup must execute it.  `dec` returns registers to the CTA's pool, `inc` waits until the pool holds
+// enough: the budgets of all warpgroups may not sum past what the kernel was launched with.
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+
 // ---------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));

@@ -1,16 +1,20 @@
 // Warp-specialised persistent GEMM / implicit-GEMM 3x3 convolution on the sm_90a warpgroup MMA (wgmma), fp16 / bf16
 // operands, fp32 accumulation.
 //
-//   grid = min(#tiles, #SMs) CTAs of 288 threads, one per SM, each looping over 128 x BN output tiles (n fastest, so the
+//   grid = min(#tiles, #SMs) CTAs of 640 threads, one per SM, each looping over 128 x BN output tiles (n fastest, so the
 //   CTAs running concurrently share A rows through L2):
-//     warp 8     : TMA producer - a ring of {A 128x64, W BNx64} 128B-swizzled k-blocks (as many stages as shared memory
-//                  holds next to the accumulator tile: 3-8)
-//     warps 0-7  : two consumer warpgroups, 64 tile rows each: wgmma m64nBNk16 straight from the ring (one k-block stays in
+//     warps 16-19: TMA producer warpgroup (one elected thread issues) - a ring of {A 128x64, W BNx64} 128B-swizzled
+//                  k-blocks (as many stages as shared memory holds next to the accumulator tile: 3-8)
+//     warps 8-15 : two MMA warpgroups, 64 tile rows each: wgmma m64nBNk16 straight from the ring (one k-block stays in
 //                  flight while the previous stage is released), then the accumulator fragments go to a row-major fp32
-//                  tile in shared memory and the same eight warps run the fused epilogue on it with one thread per tile
-//                  row: per-column parameters are per-lane constants, and a swizzled 4 KB patch per warp transposes the
-//                  result for fully coalesced 16 B loads / stores (residual / skip tensors / output).
-//   The producer streams the next tile's k-blocks while the epilogue drains the current one.
+//                  tile in shared memory (s_acc)
+//     warps 0-7  : two epilogue warpgroups run the fused epilogue on s_acc with one thread per tile row: per-column
+//                  parameters are per-lane constants, and a swizzled 4 KB patch per warp transposes the result for fully
+//                  coalesced 16 B loads / stores (residual / skip tensors / output).
+//   s_acc is handed over with two mbarriers: acc_full (fragments stored) and acc_empty (every epilogue thread has loaded
+//   its last columns).  The MMA warps wait for acc_empty only when the next tile's main loop is done, so the epilogue of
+//   tile t runs while the tensor cores work on tile t+1.  setmaxnreg moves registers from the producer (32) to the
+//   epilogue (128); the MMA warps keep the 96 of the launch.
 //   Convolution mode: A tiles are 4-D TMA boxes of the NHWC image (9 taps x channel blocks, OOB = zero padding).
 #include "common.cuh"
 #include "../../include/dinounet_b200.h"
@@ -34,8 +38,16 @@ template <int BN, int EPI = 0> struct Cfg2 {
   static constexpr int kFixed = kAccBytes + kStagingBytes + kBiasBytes + kRope + 1024 /*align*/ + 256 /*barriers*/;
   static constexpr int kStages = (kSmemMax - kFixed) / kStageBytes > 8 ? 8 : (kSmemMax - kFixed) / kStageBytes;
   static constexpr int kSmem = kStages * kStageBytes + kFixed;
-  static constexpr int kConsumerWarps = 8;
-  static constexpr int kThreads = 32 * kConsumerWarps + 32;   // two consumer warpgroups + the producer warp
+  static constexpr int kEpiWarps = 8;                          // warps 0-7: two epilogue warpgroups
+  static constexpr int kMmaWarps = 8;                          // warps 8-15: two MMA warpgroups
+  static constexpr int kThreads = 32 * (kEpiWarps + kMmaWarps) + 128;   // + the producer warpgroup (warps 16-19)
+  // Registers per thread of each role (setmaxnreg).  The launch gives every thread 65536 / 640 -> 96, and the warpgroups
+  // only trade registers among themselves: 32 + 2 x 96 + 2 x 128 = 5 x 96.
+  static constexpr int kRegLaunch = 96;
+  static constexpr int kRegProducer = 32;
+  static constexpr int kRegMma = 96;
+  static constexpr int kRegEpi = 128;
+  static_assert(kRegProducer + 2 * kRegMma + 2 * kRegEpi <= 5 * kRegLaunch, "register budget");
   static_assert(kStages >= 3, "shared-memory budget");
 };
 
@@ -154,6 +166,8 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI>::kThreads), 1) gemm_tc2_kernel(
   float* s_rope = reinterpret_cast<float*>(staging + C::kStagingBytes + C::kBiasBytes);   // [h+w][2*hq + 4] = (sin | cos | pad)
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + C::kStagingBytes + C::kBiasBytes + C::kRope);
   uint64_t* empty_bar = full_bar + 8;
+  uint64_t* acc_full = empty_bar + 8;    // s_acc holds a finished tile: every MMA thread has stored its fragments
+  uint64_t* acc_empty = acc_full + 1;    // s_acc may be overwritten: every epilogue thread has loaded what it needs
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -162,8 +176,10 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI>::kThreads), 1) gemm_tc2_kernel(
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&maps.a[0]);
     tma_prefetch_desc(&maps.b);
-    // a stage is free again once every consumer warp has seen the MMAs that read it complete
-    for (int s = 0; s < 8; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], C::kConsumerWarps); }
+    // a stage is free again once every MMA warp has seen the MMAs that read it complete
+    for (int s = 0; s < 8; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], C::kMmaWarps); }
+    mbar_init(acc_full, 32 * C::kMmaWarps);
+    mbar_init(acc_empty, 32 * C::kEpiWarps);
     fence_mbar_init();
   }
   if constexpr (EPI == 2) {
@@ -185,9 +201,10 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI>::kThreads), 1) gemm_tc2_kernel(
   __syncthreads();
   pdl_wait();                              // barriers and tensor maps are set up: now wait for the producer kernel's data
 
-  if (warp == C::kConsumerWarps) {
-    // ===================== TMA producer =====================
-    if (elect_one()) {
+  if (warp >= C::kEpiWarps + C::kMmaWarps) {
+    // ===================== TMA producer: one elected thread of warp 16 =====================
+    setmaxnreg_dec<C::kRegProducer>();
+    if (warp == C::kEpiWarps + C::kMmaWarps && elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
       for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -225,23 +242,16 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI>::kThreads), 1) gemm_tc2_kernel(
         }
       }
     }
-  } else {
-    // ===================== consumer warpgroups: MMA, then the epilogue =====================
-    const int wg = warp >> 2;                        // tile rows [64 wg, 64 wg + 64) of the MMA
-    const int q4 = warp & 3;                         // epilogue: tile rows [32 q4, 32 q4 + 32), one per lane
-    const int ew = warp;                             // staging patch index
-    const int half = warp >> 2;                      // which half of the tile's columns this warp drains
-    const int arow = q4 * 32 + lane;
-    uint8_t* patch = staging + ew * 4096;
-    const uint32_t patch_u32 = smem_u32(patch);
+  } else if (warp >= C::kEpiWarps) {
+    // ===================== MMA warpgroups: main loop, then the fragments go to s_acc =====================
+    if constexpr (C::kRegMma > C::kRegLaunch) setmaxnreg_inc<C::kRegMma>();
+    else if constexpr (C::kRegMma < C::kRegLaunch) setmaxnreg_dec<C::kRegMma>();
+    const int wg = (warp - C::kEpiWarps) >> 2;       // tile rows [64 wg, 64 wg + 64) of the MMA
+    const int q4 = warp & 3;
     const uint32_t acc_u32 = smem_u32(s_acc);
-    const b2u_epilogue& e = args.epi;
-    const int etid = threadIdx.x;                    // 0..255 among epilogue threads
     int stage = 0;
-    uint32_t phase = 0;
+    uint32_t phase = 0, acc_phase = 0;
     for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const int nt = static_cast<int>(tile % args.n_tiles);
-      const int mt = static_cast<int>(tile / args.n_tiles);
       float acc[BN / 2];
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
@@ -263,8 +273,8 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI>::kThreads), 1) gemm_tc2_kernel(
       }
       wgmma_wait<0>();
       if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
-      // accumulator fragments -> s_acc (row-major fp32)
-      epi_bar_sync();                                // the previous tile's epilogue has finished reading s_acc
+      // accumulator fragments -> s_acc (row-major fp32), once the previous tile's epilogue has loaded its part of it
+      mbar_wait(acc_empty, acc_phase ^ 1);
       {
         const int r0 = wg * 64 + q4 * 16 + (lane >> 2);
 #pragma unroll
@@ -274,7 +284,31 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI>::kThreads), 1) gemm_tc2_kernel(
           asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(acc_u32 + acc_off<BN>(r0 + 8, c)), "f"(acc[4 * j + 2]), "f"(acc[4 * j + 3]) : "memory");
         }
       }
-      epi_bar_sync();
+      mbar_arrive(acc_full);
+      acc_phase ^= 1;
+    }
+  } else {
+    // ===================== epilogue warpgroups: the fused epilogue of the tile in s_acc =====================
+    if constexpr (C::kRegEpi > C::kRegLaunch) setmaxnreg_inc<C::kRegEpi>();
+    else if constexpr (C::kRegEpi < C::kRegLaunch) setmaxnreg_dec<C::kRegEpi>();
+    const int q4 = warp & 3;                         // tile rows [32 q4, 32 q4 + 32), one per lane
+    const int ew = warp;                             // staging patch index
+    const int half = warp >> 2;                      // which half of the tile's columns this warp drains
+    const int arow = q4 * 32 + lane;
+    uint8_t* patch = staging + ew * 4096;
+    const uint32_t patch_u32 = smem_u32(patch);
+    const uint32_t acc_u32 = smem_u32(s_acc);
+    const b2u_epilogue& e = args.epi;
+    const int etid = threadIdx.x;                    // 0..255 among epilogue threads
+    uint32_t acc_phase = 0;
+    // s_acc back to the MMA warps: right after this thread's last load from it, so that the next tile's fragments can be
+    // stored while the last columns are still being processed
+    auto release_acc = [&]() { mbar_arrive(acc_empty); };
+    for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      const int nt = static_cast<int>(tile % args.n_tiles);
+      const int mt = static_cast<int>(tile / args.n_tiles);
+      mbar_wait(acc_full, acc_phase);
+      acc_phase ^= 1;
       const int n0 = nt * BN;
       int img = 0, y0 = 0, x0 = 0;
       if (args.conv) {
@@ -335,6 +369,7 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI>::kThreads), 1) gemm_tc2_kernel(
           uint32_t v0[32], v1r[32];
           acc_ld32(acc_u32, arow, hcol + lo_off, v0);
           acc_ld32(acc_u32, arow, hcol + hi_off, v1r);
+          if (u + 1 == (half + 1) * (BN / 128)) release_acc();
           const int n = n0 + hcol;
           if (n >= args.N) continue;   // warp-uniform
           const int which = n / args.D;
@@ -441,6 +476,7 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI>::kThreads), 1) gemm_tc2_kernel(
           uint32_t v0[32], v1r[32];
           acc_ld32(acc_u32, arow, g * 64, v0);
           acc_ld32(acc_u32, arow, g * 64 + 32, v1r);
+          if (g + 1 == (half + 1) * (BN / 128)) release_acc();
           const int n = n0 + g * 64;
           if (n >= args.N) continue;   // warp-uniform
           uint32_t packed[16];
@@ -529,12 +565,21 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI>::kThreads), 1) gemm_tc2_kernel(
         constexpr int kPerHalf = kChunks >= 2 ? kChunks / 2 : 1;
         const int ch_begin = kChunks >= 2 ? half * kPerHalf : 0;
         const int ch_end = kChunks >= 2 ? ch_begin + kPerHalf : (half == 0 ? 1 : 0);   // BN 32: the first warp set takes the only chunk
+        if (ch_begin == ch_end) release_acc();
 #pragma unroll 1
         for (int ch = ch_begin; ch < ch_end; ++ch) {
           uint32_t v[32];
           acc_ld32(acc_u32, arow, ch * 32, v);
+          if (ch + 1 == ch_end) release_acc();
           const int n = n0 + ch * 32;
-          const bool live = n < args.N;   // warp-uniform
+          if (n >= args.N) continue;   // warp-uniform
+          // stage raw fp32 accumulators: row = lane, 8 x 16 B groups at position j ^ (row & 7).  Done before the operand
+          // loads below so that v[] is dead by then, which keeps the epilogue inside its 128 registers.
+          __syncwarp();
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            sts128(patch_u32 + lane * 128 + ((j ^ (lane & 7)) << 4), v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+          __syncwarp();
           int ocol = n + lcol;
           long long radd = 0;
           if (e.ps_cout > 0) {
@@ -546,7 +591,7 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI>::kThreads), 1) gemm_tc2_kernel(
           // ---- prefetch residual / skip operands for every pass of this chunk
           float4 res[8];
           uint4 add[4];
-          if (live && e.residual) {
+          if (e.residual) {
             if (o32) {
 #pragma unroll
               for (int i = 0; i < 8; ++i) res[i] = *reinterpret_cast<const float4*>(e.residual + (rbase[i] + radd) * e.ldres + ocol);
@@ -558,7 +603,7 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI>::kThreads), 1) gemm_tc2_kernel(
               }
             }
           }
-          if (live && e.add16) {
+          if (e.add16) {
             if (o32) {
 #pragma unroll
               for (int i = 0; i < 4; ++i) {   // two passes per register (uint2 each)
@@ -577,21 +622,12 @@ __global__ void __launch_bounds__((Cfg2<BN, EPI>::kThreads), 1) gemm_tc2_kernel(
           float bi[NV], sc[NV], sh[NV];
 #pragma unroll
           for (int j = 0; j < NV; ++j) { bi[j] = 0.f; sc[j] = 1.f; sh[j] = 0.f; }
-          if (live) {
 #pragma unroll
-            for (int h = 0; h < NV / 4; ++h) {
-              if (e.bias) { const float4 t = __ldg(reinterpret_cast<const float4*>(e.bias + n + lcol + 4 * h)); bi[4 * h] = t.x; bi[4 * h + 1] = t.y; bi[4 * h + 2] = t.z; bi[4 * h + 3] = t.w; }
-              if (e.scale) { const float4 t = __ldg(reinterpret_cast<const float4*>(e.scale + n + lcol + 4 * h)); sc[4 * h] = t.x; sc[4 * h + 1] = t.y; sc[4 * h + 2] = t.z; sc[4 * h + 3] = t.w; }
-              if (e.shift) { const float4 t = __ldg(reinterpret_cast<const float4*>(e.shift + n + lcol + 4 * h)); sh[4 * h] = t.x; sh[4 * h + 1] = t.y; sh[4 * h + 2] = t.z; sh[4 * h + 3] = t.w; }
-            }
+          for (int h = 0; h < NV / 4; ++h) {
+            if (e.bias) { const float4 t = __ldg(reinterpret_cast<const float4*>(e.bias + n + lcol + 4 * h)); bi[4 * h] = t.x; bi[4 * h + 1] = t.y; bi[4 * h + 2] = t.z; bi[4 * h + 3] = t.w; }
+            if (e.scale) { const float4 t = __ldg(reinterpret_cast<const float4*>(e.scale + n + lcol + 4 * h)); sc[4 * h] = t.x; sc[4 * h + 1] = t.y; sc[4 * h + 2] = t.z; sc[4 * h + 3] = t.w; }
+            if (e.shift) { const float4 t = __ldg(reinterpret_cast<const float4*>(e.shift + n + lcol + 4 * h)); sh[4 * h] = t.x; sh[4 * h + 1] = t.y; sh[4 * h + 2] = t.z; sh[4 * h + 3] = t.w; }
           }
-          if (!live) continue;
-          // stage raw fp32 accumulators: row = lane, 8 x 16 B groups at position j ^ (row & 7)
-          __syncwarp();
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            sts128(patch_u32 + lane * 128 + ((j ^ (lane & 7)) << 4), v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-          __syncwarp();
           if constexpr (o32) {
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
