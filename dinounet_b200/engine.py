@@ -33,6 +33,14 @@ def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
     return None if t is None else t.data_ptr()
 
 
+def _patch_qkv_rope(args, sin: int, cos: int, keep: list):
+    """b2u_qkv_rope's arguments with other RoPE tables (a copy of its parameter block)."""
+    qp = L.QkvParams.from_buffer_copy(args[0]._obj)
+    qp.rope_sin, qp.rope_cos = sin, cos
+    keep.append(qp)
+    return (C.byref(qp),)
+
+
 class Plan:
     """A recorded sequence of C-ABI calls with their (kept-alive) arguments."""
 
@@ -40,6 +48,9 @@ class Plan:
         self.calls: List[Tuple[str, object, tuple]] = []
         self.keep: list = []
         self.vit_end = 0        # calls[:vit_end] = the frozen ViT (patch embed .. taps); calls[vit_end:] = adapter/FAPM/decoder
+        # (call index, ViT block, patch(args, sin_ptr, cos_ptr, keep) -> args) for every call that reads the RoPE tables
+        self.rope_sites: list = []
+        self.scaled_vit = None  # (Plan, scales buffer): the ViT section on per-block rescaled RoPE tables, built on first use
 
     def add(self, name: str, fn, *args):
         self.calls.append((name, fn, args))
@@ -332,6 +343,7 @@ class ForwardEngine:
             qp.v_transposed, qp.npad = 1, npad
             qp.rope_w = h
             plan.keep.append(qp)
+            plan.rope_sites.append((len(plan.calls), i, _patch_qkv_rope))
             plan.add(f"b{i}.qkv", lib.b2u_qkv_rope, C.byref(qp))
             # one launch over all ntok query rows (the 5 cls/storage rows form a ninth query tile whose out-of-range row
             # quarters only run the barrier protocol; b2u_attention_rows remains available for a split launch)
@@ -606,16 +618,54 @@ class ForwardEngine:
         return bufs["logits"], bufs["labels"]
 
     # ------------------------------------------------------------------ frozen-ViT feature caching (SURVEY.md 8f rank 3)
-    def extract_vit_features(self, x: torch.Tensor, use_graph: bool = False) -> List[torch.Tensor]:
+    def scaled_vit_plan(self, B: int, S: int) -> Tuple[Plan, torch.Tensor]:
+        """The ViT section of the (B, S) plan on per-block RoPE tables (the reference's train-mode coordinate rescaling,
+        rope_position_encoding.py:93-97, drawn once per block, vision_transformer.py:271-272): one b2u_rope_tables launch
+        fills [depth, P, head_dim] sin / cos from the returned `scales` buffer [depth], then the plan's own ViT calls run with
+        each block's RoPE pointers moved to its slice.  Shares every activation buffer of the (B, S) plan; the eval launch
+        list and its CUDA graphs are untouched."""
+        plan, _ = self.get_plan(B, S)
+        if plan.scaled_vit is None:
+            h, depth, hd = S // 16, self.v.depth, self.hd
+            dev = self.device
+            scales = torch.ones(depth, dtype=torch.float32, device=dev)
+            periods = self._dev(self.w["periods"])
+            sin = torch.empty((depth, h * h, hd), dtype=torch.float32, device=dev)
+            cos = torch.empty_like(sin)
+            sp = Plan()
+            sp.keep += [scales, periods, sin, cos]
+            sp.add("rope_tables", self.lib.b2u_rope_tables, _ptr(periods), _ptr(scales), _ptr(sin), _ptr(cos), depth, h, h, hd)
+            sites = {idx: (blk, patch) for idx, blk, patch in plan.rope_sites}
+            for idx, (name, fn, args) in enumerate(plan.calls[:plan.vit_end]):
+                if idx in sites:
+                    blk, patch = sites[idx]
+                    args = patch(args, sin[blk].data_ptr(), cos[blk].data_ptr(), sp.keep)
+                sp.calls.append((name, fn, args))
+            assert len(sites) == depth
+            plan.scaled_vit = (sp, scales)
+        return plan.scaled_vit
+
+    def extract_vit_features(self, x: torch.Tensor, use_graph: bool = False,
+                             rope_scales: Optional[torch.Tensor] = None) -> List[torch.Tensor]:
         """The four tapped, final-LayerNorm'ed ViT outputs [B, P, D] (fp32) of the FROZEN backbone
         (dinov3_adapter.py:422-426: `with torch.no_grad()` around get_intermediate_layers).  In eval mode they depend only
         on the image, so a caller that sees a sample repeatedly (every training epoch, every mirrored / overlapping
         sliding-window pass over the same tile) may cache them and skip 57-88 % of the forward FLOPs with
-        `forward_from_vit_features`.  Returns fresh tensors (not the engine's buffers)."""
+        `forward_from_vit_features`.  rope_scales [depth] (fp32): block i's RoPE coordinates are multiplied by
+        rope_scales[i] (the reference's train mode; runs `scaled_vit_plan`, without a CUDA graph).  Returns fresh tensors
+        (not the engine's buffers)."""
         B, _, S, _ = x.shape
         plan, bufs = self.get_plan(B, S)
         bufs["x"].copy_(x, non_blocking=True)
-        self.run_resident(B, S, use_graph, part="vit")
+        if rope_scales is None:
+            self.run_resident(B, S, use_graph, part="vit")
+        else:
+            if tuple(rope_scales.shape) != (self.v.depth,):
+                raise ValueError(f"rope_scales must have shape [{self.v.depth}], got {tuple(rope_scales.shape)}")
+            sp, scales = self.scaled_vit_plan(B, S)
+            scales.copy_(rope_scales, non_blocking=True)
+            with torch.cuda.device(self.device):
+                sp.run(torch.cuda.current_stream(self.device).cuda_stream)
         P = (S // 16) ** 2
         return [bufs[f"tap{k}"].view(B, P, -1).clone() for k in range(4)]
 

@@ -21,6 +21,11 @@ def _ptr(t):
     return None if t is None else t.data_ptr()
 
 
+def _patch_attention_rope(args, sin: int, cos: int, keep: list):
+    """b2u_f32_attention's arguments (qkv, sin, cos, out, ...) with other RoPE tables."""
+    return (args[0], sin, cos) + tuple(args[3:])
+
+
 def build_plan_fp32(eng, B: int, S: int):
     from .engine import Plan
     if S % 32 or S < 64:
@@ -92,6 +97,7 @@ def build_plan_fp32(eng, B: int, S: int):
     for i in range(v.depth):
         ln(f"b{i}.ln1", X, Y, f"b{i}.n1w", f"b{i}.n1b", T, cfg.LN_EPS_VIT)
         gemm(f"b{i}.qkv", Y, T, D, D, w[f"b{i}.qkv"], 3 * D, QKV, 3 * D, bias=w.get(f"b{i}.qkvb"))
+        plan.rope_sites.append((len(plan.calls), i, _patch_attention_rope))
         plan.add(f"b{i}.attn", lib.b2u_f32_attention, _ptr(QKV), _ptr(sin), _ptr(cos), _ptr(O), B, N, Hh, hd, cfg.N_PREFIX,
                  hd ** -0.5)
         gemm(f"b{i}.proj", O, T, D, D, w[f"b{i}.proj"], D, X, D, bias=w[f"b{i}.projb"], scale=w[f"b{i}.ls1"], residual=X, ldres=D)

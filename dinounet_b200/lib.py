@@ -147,13 +147,21 @@ SIGNATURES = {
     "b2u_f32_conv3x3_wgrad": [vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp],
     "b2u_f32_sqsum": [vp, i64, vp, vp],
     "b2u_f32_sgd_nesterov": [vp, vp, vp, i64, f32, f32, f32, vp, f32, i32, vp],
+    "b2u_f32_bn_work_doubles": [i64, i32],
+    "b2u_f32_bn_stats": [vp, i64, i32, vp, vp, vp],
+    "b2u_f32_bn_finalize": [vp, i32, vp, vp, vp, vp, vp, f32, vp],
+    "b2u_f32_bn_train_bwd_reduce": [vp, vp, vp, vp, vp, vp, f32, i64, i32, i32, vp, vp, vp, vp, vp],
+    "b2u_f32_bn_train_bwd_apply": [vp, vp, vp, vp, vp, vp, f32, vp, vp, i64, i32, i32, vp],
+    "b2u_f32_droppath_add": [vp, vp, vp, vp, i64, i32, i64, vp],
+    "b2u_rope_tables": [vp, vp, vp, vp, i32, i32, i32, i32, vp],
     "b2u_set_option": [i32, i32],
     "b2u_last_error": [],
     "b2u_version": [],
     "b2u_launch_count": [],
 }
 _RESTYPES = {"b2u_last_error": C.c_char_p, "b2u_launch_count": C.c_int64, "b2u_in_stats_work_floats": C.c_int64,
-             "b2u_dice_ce_work_doubles": C.c_int64, "b2u_dice_bce_work_doubles": C.c_int64}
+             "b2u_dice_ce_work_doubles": C.c_int64, "b2u_dice_bce_work_doubles": C.c_int64,
+             "b2u_f32_bn_work_doubles": C.c_int64}
 
 _lib: Optional[C.CDLL] = None
 

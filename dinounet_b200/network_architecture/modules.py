@@ -504,6 +504,12 @@ class DinoUNet(nn.Module):
     #: accumulation (default; the reference trains under fp16 autocast = the same mantissa); "fp32" = IEEE-fp32 SIMT kernels
     #: (the tier the gradient goldens are held to at 2e-3)
     train_gemm = "tf32"
+    #: what `.train()` means for the training step.  "oracle" (default) = eval-mode modules in both module modes: BatchNorm
+    #: on running statistics (never updated), DropPath off, the ViT's RoPE unscaled - the semantics the gradient goldens pin.
+    #: "reference" = the reference's train mode: batch-statistics SyncBatchNorm that updates running_mean / running_var /
+    #: num_batches_tracked (all-reduced across the ranks of the default process group), DropPath(0.3) on the extractors'
+    #: ConvFFN branch and a log-uniform RoPE coordinate factor in [1/2, 2] per ViT block (see `train_forward`)
+    train_semantics = "oracle"
 
     def __init__(self, network_config: dict = None, input_channels: int = None, num_classes: int = None,
                  dinov3_pretrained_path: str = "dinounet/checkpoints/dinov3_vits16_pretrain_lvd1689m-08c60483.pth",
@@ -558,6 +564,7 @@ class DinoUNet(nn.Module):
         self.decoder = UNetDecoder(self.encoder, num_classes, n_conv_per_stage_decoder, deep_supervision,
                                    nonlin_first=nonlin_first)
         self._engine = None
+        self._repack_before_eval = False
         self.register_load_state_dict_post_hook(lambda module, incompatible: module._invalidate())
 
     def _create_dinov3_encoder(self, pretrained_path, model_name, features_per_stage, conv_op, norm_op, norm_op_kwargs,
@@ -587,6 +594,15 @@ class DinoUNet(nn.Module):
     def repack(self):
         """Call after mutating parameters in place (e.g. an optimizer step) to refresh the packed kernel weights."""
         self._engine = None
+
+    def _eval_engine(self, device):
+        """The engine for eval-path entries.  A "reference"-semantics train forward changes the BatchNorm running statistics
+        (and an optimizer step usually follows it), and the engine folds BatchNorm into its packed weights, so the first
+        eval entry after one repacks."""
+        if self._repack_before_eval:
+            self._engine = None
+            self._repack_before_eval = False
+        return self._get_engine(device)
 
     def _check_block_spec(self):
         """The conv blocks are compiled for Conv2d(3x3, bias) -> InstanceNorm2d(eps 1e-5, affine) -> LeakyReLU(0.01), two
@@ -633,9 +649,8 @@ class DinoUNet(nn.Module):
                                       "(DinoUNetTrainer derives from nnUNetTrainerNoDeepSupervision)")
         if torch.is_grad_enabled() and self.training:
             # training step (nnUNetTrainer.py:899-929): frozen ViT on the engine, everything else differentiable through the
-            # autograd Functions of train_path.py (forward and backward on hand-written kernels; `train_gemm` picks the matrix-product tier).  Semantics of the
-            # gradient oracle: BatchNorm uses running statistics and DropPath is off in BOTH module modes (the reference's
-            # train-mode stochasticity of the frozen ViT, SURVEY.md fact 8, is deliberately not reproduced).
+            # autograd Functions of train_path.py (forward and backward on hand-written kernels; `train_gemm` picks the
+            # matrix-product tier, `train_semantics` eval-mode modules ("oracle") or the reference's train mode)
             return self.train_forward(x)
         B, Cc, H, W = x.shape
         if Cc == 1:                       # dinounet_training.py:491-497
@@ -643,26 +658,88 @@ class DinoUNet(nn.Module):
         elif Cc != 3:
             x = x.repeat(1, 3 // Cc + (1 if 3 % Cc != 0 else 0), 1, 1)[:, :3] if Cc < 3 else x[:, :3]
         x = x.float().contiguous()
-        logits, _ = self._get_engine(x.device).forward(x)
+        logits, _ = self._eval_engine(x.device).forward(x)
         return logits.clone()
 
-    def train_forward(self, x: torch.Tensor) -> torch.Tensor:
-        """Differentiable logits [B, C, H, W] (fp32): gradients for the 289 trainable tensors outside the frozen backbone."""
-        from ..train_path import trainable_forward
+    #: the reference's order of the six extractors (the rows of `drop_keep`) and the keep probability of their DropPath
+    _EXTRACTORS = [f"encoder.dinov3_adapter.interactions.{i}.extractor" for i in range(4)] + \
+        [f"encoder.dinov3_adapter.interactions.3.extra_extractors.{j}" for j in range(2)]
+    _DROP_KEEP = 0.7
+
+    def _train_bn_config(self):
+        """(momentum, eps) of the ten SyncBatchNorm layers, keyed by their state-dict prefix."""
+        out = {}
+        for name, m in self.named_modules():
+            if not isinstance(m, nn.modules.batchnorm._BatchNorm) or name.startswith("decoder.encoder."):
+                continue
+            if m.momentum is None or not m.track_running_stats:
+                raise NotImplementedError(f"{name}: train_semantics='reference' implements BatchNorm with a momentum and "
+                                          f"running statistics (momentum={m.momentum}, "
+                                          f"track_running_stats={m.track_running_stats})")
+            out[name] = (float(m.momentum), float(m.eps))
+        return out
+
+    def _draw_train_randomness(self, batch: int, device, scales: bool = True, keep: bool = True):
+        """(rope_scales [depth], drop_keep [6, batch]) from torch's default generator of `device`, in the reference's order
+        (one RoPE factor exp(U(-ln 2, ln 2)) per ViT block, then the extractors' Bernoulli(0.7) keep flags); a part not
+        asked for is None and draws nothing."""
+        depth = cfg.VARIANTS[self.dinov3_model_name].depth
+        s = k = None
+        if scales:
+            s = torch.empty(depth, dtype=torch.float32, device=device).uniform_(-math.log(2.0), math.log(2.0)).exp_()
+        if keep:
+            k = torch.empty((len(self._EXTRACTORS), batch), dtype=torch.float32, device=device).bernoulli_(self._DROP_KEEP)
+        return s, k
+
+    def train_forward(self, x: torch.Tensor, *, rope_scales: torch.Tensor = None, drop_keep: torch.Tensor = None) -> torch.Tensor:
+        """Differentiable logits [B, C, H, W] (fp32): gradients for the 289 trainable tensors outside the frozen backbone.
+        With train_semantics == "reference", `rope_scales` [depth] (fp32 RoPE coordinate factor of each ViT block) and
+        `drop_keep` [6, B] (0/1 DropPath keep flags, one row per extractor in the order interactions.0..3.extractor,
+        interactions.3.extra_extractors.0..1) pin the random draws; an absent one is drawn on the model's device from
+        torch's default CUDA generator: exp(U(-ln 2, ln 2)) per block, Bernoulli(0.7) per flag.  Both are ignored by
+        "oracle"."""
+        from ..train_path import TrainMode, _bn_sync, trainable_forward
+        sem = self.train_semantics
+        if sem not in ("oracle", "reference"):
+            raise ValueError(f"train_semantics must be 'oracle' or 'reference', got {sem!r}")
+        if sem == "reference":
+            if self.dinov3_model_name.startswith("dinounet_7b"):
+                raise NotImplementedError("train_semantics='reference' does not cover dinounet_7b: its ViT's train-mode "
+                                          "batch-subset stochastic depth (drop_path_rate 0.4) is not implemented")
+            bn = self._train_bn_config()
         if x.device.type != "cuda":
             from ..lib import NativeLibraryError
             raise NativeLibraryError("dinounet_b200 runs on CUDA devices only (no CPU fallback)")
         x = self._three_channels(x)
+        gemm = getattr(self, "train_gemm", "tf32")
+        if sem == "oracle":
+            with torch.no_grad():
+                taps = self._get_engine(x.device).extract_vit_features(x)
+            P = self.state_dict(keep_vars=True)
+            return trainable_forward(P, self.dinov3_model_name, x, taps, self.num_classes, gemm)
+        B = x.shape[0]
+        depth = cfg.VARIANTS[self.dinov3_model_name].depth
         with torch.no_grad():
-            taps = self._get_engine(x.device).extract_vit_features(x)
+            if rope_scales is None or drop_keep is None:
+                drawn = self._draw_train_randomness(B, x.device, rope_scales is None, drop_keep is None)
+                rope_scales = drawn[0] if rope_scales is None else rope_scales
+                drop_keep = drawn[1] if drop_keep is None else drop_keep
+            rope_scales = rope_scales.to(device=x.device, dtype=torch.float32).contiguous()
+            drop_keep = drop_keep.to(device=x.device, dtype=torch.float32)
+            if tuple(rope_scales.shape) != (depth,) or tuple(drop_keep.shape) != (len(self._EXTRACTORS), B):
+                raise ValueError(f"rope_scales must be [{depth}] and drop_keep [{len(self._EXTRACTORS)}, {B}], got "
+                                 f"{tuple(rope_scales.shape)} and {tuple(drop_keep.shape)}")
+            taps = self._get_engine(x.device).extract_vit_features(x, rope_scales=rope_scales)
         P = self.state_dict(keep_vars=True)
-        return trainable_forward(P, self.dinov3_model_name, x, taps, self.num_classes, getattr(self, "train_gemm", "tf32"))
+        mode = TrainMode(bn=bn, drop_scale=(drop_keep / self._DROP_KEEP).contiguous(), sync=_bn_sync())
+        self._repack_before_eval = True
+        return trainable_forward(P, self.dinov3_model_name, x, taps, self.num_classes, gemm, mode)
 
     @torch.no_grad()
     def predict_labels(self, x: torch.Tensor) -> torch.Tensor:
         """argmax mask (uint8) straight from the fused seg-head kernel (nnUNetTrainer.py:977)."""
         x = x.float().contiguous()
-        _, labels = self._get_engine(x.device).forward(x)
+        _, labels = self._eval_engine(x.device).forward(x)
         return labels.clone()
 
     # ---- frozen-backbone feature caching (SURVEY.md section 8f rank 3) --------------------------------------------
@@ -679,13 +756,13 @@ class DinoUNet(nn.Module):
         """The frozen DINOv3 backbone's four tapped token maps [B, P, D] for `x` (eval mode: a pure function of the image,
         dinov3_adapter.py:422-426) - cache them per sample and feed `forward_from_vit_features` to skip the ViT."""
         x = self._three_channels(x)
-        return self._get_engine(x.device).extract_vit_features(x)
+        return self._eval_engine(x.device).extract_vit_features(x)
 
     @torch.no_grad()
     def forward_from_vit_features(self, x: torch.Tensor, feats) -> torch.Tensor:
         """Logits from the image plus cached backbone features: runs only SPM + extractors + FAPM + decoder."""
         x = self._three_channels(x)
-        logits, _ = self._get_engine(x.device).forward_from_vit_features(x, feats)
+        logits, _ = self._eval_engine(x.device).forward_from_vit_features(x, feats)
         return logits.clone()
 
     def compute_conv_feature_map_size(self, input_size):

@@ -15,15 +15,18 @@ head (289 tensors).  Here:
     with ONE parameter block: `gemm="tf32"` (default) = `b2u_tf32_gemm`, wgmma tensor cores with TF32-rounded operands
     and fp32 accumulation (the mantissa of the fp16 autocast the reference trains under); `gemm="fp32"` = `b2u_f32_gemm`,
     the IEEE-fp32 SIMT kernel the gradient goldens are held to at 2e-3.  Everything else is fp32 in both tiers;
-  * semantics = the gradient oracle's (oracle/grad_oracle.py, pinned to autograd through the REAL reference): eval-mode
-    BatchNorm (running statistics), DropPath off, fp32.
+  * semantics (`DinoUNet.train_semantics`): "oracle" (default) = the gradient oracle's (oracle/grad_oracle.py, pinned to
+    autograd through the REAL reference): eval-mode BatchNorm (running statistics), DropPath off, fp32.  "reference" = the
+    reference's train mode (`TrainMode`): batch-statistics SyncBatchNorm with the running-statistic update, DropPath on the
+    extractors' ConvFFN branch, and the ViT taps computed with per-block rescaled RoPE coordinates (engine.py).
 
 Layout: activations are 2-D fp32 tensors [rows, C] (tokens, or NHWC pixels), exactly the fp32 tier's.
 """
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict, List, Optional
+from dataclasses import dataclass
+from typing import Dict, List, Optional, Tuple
 
 import torch
 from torch.autograd import Function
@@ -260,6 +263,80 @@ class BNActF(Function):
         return (dx if ctx.needs_input_grad[0] else None), dg, db, None, None, None
 
 
+def _bn_sync() -> bool:
+    """torch SyncBatchNorm's `need_sync`: train mode under an initialised default process group of more than one rank."""
+    dist = torch.distributed
+    return bool(dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1)
+
+
+class BNTrainF(Function):
+    """train-mode (Sync)BatchNorm + optional ReLU on [rows, C]: normalises with the batch mean and biased variance and
+    updates running_mean / running_var / num_batches_tracked in place (torch SyncBatchNorm.forward in train mode).  With
+    `sync`, the per-channel sums and the row count are all-reduced on the current stream before the finalize, and the
+    backward's sum dy' and sum dy' xhat before dx; dgamma / dbeta stay local (DDP averages them)."""
+
+    @staticmethod
+    def forward(ctx, x, gamma, beta, rm, rv, nbt, act, momentum, eps, sync):
+        x = x.contiguous()
+        rows, Cc = x.shape
+        if rows < 2:
+            raise ValueError(f"BatchNorm in train mode needs more than 1 value per channel, got {rows} rows")
+        dev = x.device
+        lib = L.load()
+        work = torch.empty(int(lib.b2u_f32_bn_work_doubles(rows, Cc)), dtype=torch.float64, device=dev)
+        sums = torch.empty(2 * Cc + 1, dtype=torch.float64, device=dev)
+        mean = torch.empty(Cc, dtype=torch.float32, device=dev)
+        var = torch.empty(Cc, dtype=torch.float32, device=dev)
+        _call("b2u_f32_bn_stats", x, rows, Cc, work, sums)
+        if sync:
+            torch.distributed.all_reduce(sums)
+        _call("b2u_f32_bn_finalize", sums, Cc, mean, var, rm, rv, nbt, float(momentum))
+        y = torch.empty_like(x)
+        _call("b2u_f32_bn_act", x, y, gamma, beta, mean, var, float(eps), rows, Cc, act)
+        ctx.save_for_backward(x, gamma, beta, mean, var)
+        ctx.cfg = (act, float(eps), bool(sync))
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, gamma, beta, mean, var = ctx.saved_tensors
+        act, eps, sync = ctx.cfg
+        dy = dy.contiguous()
+        rows, Cc = x.shape
+        dev = x.device
+        work = torch.empty(int(L.load().b2u_f32_bn_work_doubles(rows, Cc)), dtype=torch.float64, device=dev)
+        red = torch.empty(2 * Cc + 1, dtype=torch.float64, device=dev)
+        dg, db = torch.empty_like(gamma), torch.empty_like(beta)
+        _call("b2u_f32_bn_train_bwd_reduce", x, dy, gamma, beta, mean, var, eps, rows, Cc, act, work, red, dg, db)
+        if sync:
+            torch.distributed.all_reduce(red)
+        dx = torch.empty_like(x)
+        _call("b2u_f32_bn_train_bwd_apply", x, dy, gamma, beta, mean, var, eps, red, dx, rows, Cc, act)
+        return dx, dg, db, None, None, None, None, None, None, None
+
+
+class DropPathAddF(Function):
+    """c + s[sample] * f on [B*rows_per_sample, D] (the extractor's `query + drop_path(ffn(...))`, per-sample scale
+    s = keep / (1 - drop_prob)); backward: dc = dy, df = s * dy."""
+
+    @staticmethod
+    def forward(ctx, c, f, s, rows_per_sample):
+        c, f = c.contiguous(), f.contiguous()
+        y = torch.empty_like(c)
+        _call("b2u_f32_droppath_add", c, f, s, y, c.shape[0], c.shape[1], rows_per_sample)
+        ctx.save_for_backward(s)
+        ctx.rps = rows_per_sample
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        (s,) = ctx.saved_tensors
+        dy = dy.contiguous()
+        df = torch.empty_like(dy)
+        _call("b2u_f32_droppath_add", None, dy, s, df, dy.shape[0], dy.shape[1], ctx.rps)
+        return dy, df, None, None
+
+
 class ActF(Function):
     @staticmethod
     def forward(ctx, x, act):
@@ -429,22 +506,34 @@ class TailAddF(Function):
 
 
 # ------------------------------------------------------------------------------------------------------------ the network
+@dataclass
+class TrainMode:
+    """The reference's train-mode semantics for one forward: `bn` maps each BatchNorm prefix of P to its (momentum, eps),
+    `drop_scale` [6, B] holds the extractors' per-sample DropPath factors keep / (1 - drop_prob), and `sync` all-reduces
+    the BatchNorm statistics across the default process group."""
+    bn: Dict[str, Tuple[float, float]]
+    drop_scale: torch.Tensor
+    sync: bool = False
+
+
 def trainable_forward(P: Dict[str, torch.Tensor], variant: str, x: torch.Tensor, taps: List[torch.Tensor], num_classes: int,
-                      gemm: str = "tf32") -> torch.Tensor:
+                      gemm: str = "tf32", train_mode: Optional[TrainMode] = None) -> torch.Tensor:
     """Differentiable forward of everything outside the frozen backbone.  P: reference-keyed parameters / buffers
     (`net.state_dict(keep_vars=True)`), x [B,3,S,S] fp32, taps: 4 x [B, P, D] fp32 (frozen ViT outputs) -> logits [B,C,S,S].
-    gemm: matrix-product tier, "tf32" (tensor cores) or "fp32" (SIMT parity tier); the backward uses the same tier."""
+    gemm: matrix-product tier, "tf32" (tensor cores) or "fp32" (SIMT parity tier); the backward uses the same tier.
+    train_mode: None = eval-mode modules (BatchNorm on running statistics, DropPath off); a TrainMode = batch-statistics
+    BatchNorm that updates the running statistics in P, and DropPath with the given factors."""
     global _GEMM_TIER
     if gemm not in ("tf32", "fp32"):
         raise ValueError(f"gemm tier must be 'tf32' or 'fp32', got {gemm!r}")
     prev, _GEMM_TIER = _GEMM_TIER, gemm
     try:
-        return _trainable_forward(P, variant, x, taps, num_classes)
+        return _trainable_forward(P, variant, x, taps, num_classes, train_mode)
     finally:
         _GEMM_TIER = prev
 
 
-def _trainable_forward(P, variant, x, taps, num_classes):
+def _trainable_forward(P, variant, x, taps, num_classes, train_mode=None):
     v = cfg.VARIANTS[variant]
     D = v.embed_dim
     B, _, S, _ = x.shape
@@ -455,7 +544,11 @@ def _trainable_forward(P, variant, x, taps, num_classes):
     Lq = n2 + n3 + n4
     A = "encoder.dinov3_adapter."
     lin = lambda t, p, res=None: LinearF.apply(t, P[p + ".weight"].reshape(P[p + ".weight"].shape[0], -1), P.get(p + ".bias"), res)
-    bn = lambda t, p, act: BNActF.apply(t, P[p + ".weight"], P[p + ".bias"], P[p + ".running_mean"], P[p + ".running_var"], act)
+    if train_mode is None:
+        bn = lambda t, p, act: BNActF.apply(t, P[p + ".weight"], P[p + ".bias"], P[p + ".running_mean"], P[p + ".running_var"], act)
+    else:
+        bn = lambda t, p, act: BNTrainF.apply(t, P[p + ".weight"], P[p + ".bias"], P[p + ".running_mean"], P[p + ".running_var"],
+                                              P[p + ".num_batches_tracked"], act, *train_mode.bn[p], train_mode.sync)
 
     # ---- SPM (dinov3_adapter.py:279-302)
     Sp = A + "spm."
@@ -491,7 +584,10 @@ def _trainable_forward(P, variant, x, taps, num_classes):
         fq = LayerNormF.apply(c, P[p + "ffn_norm.weight"], P[p + "ffn_norm.bias"], cfg.LN_EPS_ADAPTER)
         f1 = lin(fq, p + "ffn.fc1")
         f2 = ActF.apply(DWConvF.apply(f1, P[p + "ffn.dwconv.dwconv.weight"], P[p + "ffn.dwconv.dwconv.bias"], B, S16, S16, 3), L.ACT_GELU)
-        c = lin(f2, p + "ffn.fc2", c)                               # c + ffn
+        if train_mode is None:
+            c = lin(f2, p + "ffn.fc2", c)                           # c + ffn
+        else:
+            c = DropPathAddF.apply(c, lin(f2, p + "ffn.fc2"), train_mode.drop_scale[e], Lq)   # c + drop_path(ffn)
 
     # ---- adapter tail (dinov3_adapter.py:460-482)
     c3d = c.view(B, Lq, D)

@@ -25,11 +25,15 @@ class DinoUNetTrainer(_Base):
     _network_config = None
     _dinov3_pretrained_path = None
     _dinov3_model_name = None
+    _train_semantics = None
 
     @classmethod
     def set_network_config(cls, network_config, dinov3_pretrained_path=None, dinov3_model_name=None,
-                           adapter_type="default"):
+                           adapter_type="default", train_semantics=None):
+        """train_semantics: `DinoUNet.train_semantics` of the networks `build_network_architecture` returns ("oracle" or
+        "reference"); None keeps the module default."""
         cls._network_config = network_config
+        cls._train_semantics = train_semantics
         if dinov3_pretrained_path is not None:
             cls._dinov3_pretrained_path = dinov3_pretrained_path
         if dinov3_model_name is not None:
@@ -38,6 +42,7 @@ class DinoUNetTrainer(_Base):
         DinoUNetTrainer._network_config = cls._network_config
         DinoUNetTrainer._dinov3_model_name = cls._dinov3_model_name
         DinoUNetTrainer._dinov3_pretrained_path = cls._dinov3_pretrained_path
+        DinoUNetTrainer._train_semantics = cls._train_semantics
 
     @staticmethod
     def build_network_architecture(architecture_class_name: str, arch_init_kwargs: dict,
@@ -49,10 +54,13 @@ class DinoUNetTrainer(_Base):
         config = DinoUNetTrainer._network_config.copy()
         config["architecture"] = config["architecture"].copy()
         config["architecture"]["deep_supervision"] = enable_deep_supervision
-        return DinoUNet.from_config(network_config=config, input_channels=num_input_channels,
-                                    num_classes=num_output_channels,
-                                    dinov3_pretrained_path=DinoUNetTrainer._dinov3_pretrained_path,
-                                    dinov3_model_name=DinoUNetTrainer._dinov3_model_name)
+        net = DinoUNet.from_config(network_config=config, input_channels=num_input_channels,
+                                   num_classes=num_output_channels,
+                                   dinov3_pretrained_path=DinoUNetTrainer._dinov3_pretrained_path,
+                                   dinov3_model_name=DinoUNetTrainer._dinov3_model_name)
+        if DinoUNetTrainer._train_semantics is not None:
+            net.train_semantics = DinoUNetTrainer._train_semantics
+        return net
 
 
     # ---- forward-only callers of the path that the trainer owns (nnUNetTrainer.py:355-365, :945-1005)

@@ -414,6 +414,38 @@ int b2u_f32_sqsum(const float* g, int64_t n, double* out_accum, b2u_stream_t str
 int b2u_f32_sgd_nesterov(float* p, const float* g, float* momentum_buf, int64_t n, float lr, float momentum, float weight_decay,
                          const double* grad_sqsum, float max_norm, int32_t first_step, b2u_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * Train-mode semantics of the reference (csrc/train_mode.cu): batch-statistics (Sync)BatchNorm with the running-statistic
+ * update, the extractors' DropPath residual and per-block RoPE tables with rescaled coordinates.  No atomics: every
+ * reduction goes through fixed-order fp64 partials, so two identical launches give identical bits.
+ *
+ * BatchNorm training step on x [rows, C] (torch SyncBatchNorm in train mode):
+ *   b2u_f32_bn_stats     sums[0:C] = sum x, sums[C:2C] = sum x^2, sums[2C] = rows (fp64; work: b2u_f32_bn_work_doubles).
+ *                        Data-parallel callers all-reduce `sums` (all 2C+1 doubles) before the finalize.
+ *   b2u_f32_bn_finalize  n = sums[2C]: batch mean and biased variance -> mean, var (fp32); running_mean/var <- (1-m)*r +
+ *                        m*(mean | var*n/(n-1)); *num_batches_tracked += 1.  Normalise with b2u_f32_bn_act(mean, var).
+ *   b2u_f32_bn_train_bwd_reduce  dy' = dy (ReLU-masked when act): red[0:C] = sum dy', red[C:2C] = sum dy' xhat,
+ *                        red[2C] = rows; dgamma = sum dy' xhat, dbeta = sum dy' (written, local).  All-reduce `red` for sync.
+ *   b2u_f32_bn_train_bwd_apply   dx = gamma*invstd*(dy' - red[c]/n - xhat*red[C+c]/n), n = red[2C]. */
+int64_t b2u_f32_bn_work_doubles(int64_t rows, int32_t C);
+int b2u_f32_bn_stats(const float* x, int64_t rows, int32_t C, double* work, double* sums, b2u_stream_t stream);
+int b2u_f32_bn_finalize(const double* sums, int32_t C, float* mean, float* var, float* running_mean, float* running_var,
+                        int64_t* num_batches_tracked, float momentum, b2u_stream_t stream);
+int b2u_f32_bn_train_bwd_reduce(const float* x, const float* dy, const float* gamma, const float* beta, const float* mean,
+                                const float* var, float eps, int64_t rows, int32_t C, int32_t act, double* work, double* red,
+                                float* dgamma, float* dbeta, b2u_stream_t stream);
+int b2u_f32_bn_train_bwd_apply(const float* x, const float* dy, const float* gamma, const float* beta, const float* mean,
+                               const float* var, float eps, const double* red, float* dx, int64_t rows, int32_t C, int32_t act,
+                               b2u_stream_t stream);
+/* DropPath residual (dinov3_adapter.py:18-27): y = c + s[row / rows_per_sample] * f over [rows, D]; c == NULL gives
+ * y = s * f (the backward of the branch). */
+int b2u_f32_droppath_add(const float* c, const float* f, const float* s, float* y, int64_t rows, int32_t D,
+                         int64_t rows_per_sample, b2u_stream_t stream);
+/* Per-block RoPE tables (rope_position_encoding.py:57-106, 'separate' coordinates times scales[i]):
+ * sin/cos [depth, h*w, head_dim] fp32 from periods [head_dim/4] and scales [depth] (device). */
+int b2u_rope_tables(const float* periods, const float* scales, float* sin, float* cos, int32_t depth, int32_t h, int32_t w,
+                    int32_t head_dim, b2u_stream_t stream);
+
 int b2u_set_option(int32_t key, int32_t value);
 
 const char* b2u_last_error(void);
