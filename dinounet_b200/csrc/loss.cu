@@ -14,6 +14,9 @@
 // batch sums [C][3] (intersect, sum_pred, sum_gt; fp64, on the device), which the caller all-reduces across ranks before
 // the finalisation.  The backward takes the incoming gradient as device scalars: the CE/BCE part is scaled by the local
 // one, the Dice part by the all-reduced one (the backward of AllGatherGrad, ddp_allgather.py:43-48).  No host sync.
+//
+// An ignore label (DC_and_CE_loss(..., ignore_label), compound_losses.py:38-53) takes the split entry points with the
+// kernels' IGN instantiations: masked sums, a valid-pixel count per sample, CE over the valid pixels only.
 #include "common.cuh"
 #include "host_util.h"
 #include "gemm_common.h"
@@ -89,13 +92,16 @@ __device__ __forceinline__ void block_sum_store(const float (&acc)[N], double* _
   }
 }
 
-template <int C>
+// IGN: pixels labelled `ignore_label` add nothing, and each sample's record gains the valid-pixel count after the CE sum
+// (RobustCrossEntropyLoss ignore_index + MemoryEfficientSoftDiceLoss loss_mask).  Their logits are read as without IGN,
+// but reach no sum.
+template <int C, bool IGN = false>
 __global__ void __launch_bounds__(256) loss_stats_kernel(const float* __restrict__ logits, const void* __restrict__ target,
                                                          int tkind, double* __restrict__ partial, int* __restrict__ bad,
-                                                         long long plane) {
+                                                         long long plane, int ignore_label) {
   const int b = blockIdx.y;
   const float* zb = logits + static_cast<long long>(b) * C * plane;
-  constexpr int K = C * kStat + 1;  // the last sum is the CE
+  constexpr int K = C * kStat + 1 + IGN;  // then the CE sum (and the valid-pixel count)
   float acc[K];
 #pragma unroll
   for (int k = 0; k < K; ++k) acc[k] = 0.f;
@@ -105,6 +111,10 @@ __global__ void __launch_bounds__(256) loss_stats_kernel(const float* __restrict
     int amax;
     pixel_softmax<C>(zb + i, plane, p, mx, lse, amax);
     int t = label_at(target, tkind, static_cast<long long>(b) * plane + i);
+    if constexpr (IGN) {
+      if (t == ignore_label) continue;
+      acc[C * kStat + 1] += 1.f;
+    }
     if (t < 0 || t >= C) { *bad = 1; t = 0; }
     acc[C * kStat] += lse - (zb[t * plane + i] - mx);
 #pragma unroll
@@ -134,33 +144,40 @@ __device__ __forceinline__ void reduce_sample_stats(const double* __restrict__ p
 
 // bsum[c][3] = (intersect, sum_pred, sum_gt) of class c over the batch: per sample in block order, then in sample
 // order, which is the order the fused finalisation sums in.  K = per-sample record length; class c's record at c*kStat.
-__global__ void dice_batch_sums_kernel(const double* __restrict__ partial, double* __restrict__ bsum, int B, int C,
-                                       int K, int nblk) {
+// The per-sample sums go through `stats` (B*K doubles) so that every thread of the block takes part in the long first
+// level, instead of one thread per output running over all B*nblk partials.
+__global__ void dice_batch_sums_kernel(const double* __restrict__ partial, double* __restrict__ stats,
+                                       double* __restrict__ bsum, int B, int C, int K, int nblk) {
+  reduce_sample_stats(partial, stats, B, K, nblk);
+  __syncthreads();
   for (int j = threadIdx.x; j < C * 3; j += blockDim.x) {
     const int c = j / 3, s = j - c * 3;
     double v = 0;
-    for (int b = 0; b < B; ++b) {
-      double vb = 0;
-      for (int n = 0; n < nblk; ++n) vb += partial[(static_cast<long long>(b) * nblk + n) * K + c * kStat + s];
-      v += vb;
-    }
+    for (int b = 0; b < B; ++b) v += stats[b * K + c * kStat + s];
     bsum[j] = v;
   }
 }
 
-// stats: double [B][C*6 + 1] (the +1 is the sample's CE sum).  out: float[3] = loss, ce, dice term.
-// gsum (optional): batch sums [C][3] to take the batch Dice from (all-reduced across data-parallel ranks).
+// stats: double [B][C*6 + 1 (+1 with IGN)] (the sample's CE sum, and its valid-pixel count).  out: float[3] = loss, ce,
+// dice term.  gsum (optional): batch sums [C][3] to take the batch Dice from (all-reduced across data-parallel ranks).
+template <bool IGN = false>
 __global__ void loss_finalize_kernel(const double* __restrict__ partial, double* __restrict__ stats,
                                      const double* __restrict__ gsum, float* __restrict__ out,
                                      int64_t* __restrict__ tpfpfn, int B, int C, int nblk, long long plane, float w_ce,
                                      float w_dice, int batch_dice, int do_bg, float smooth) {
-  const int K = C * kStat + 1;
+  const int K = C * kStat + 1 + IGN;
   reduce_sample_stats(partial, stats, B, K, nblk);
   __syncthreads();
   if (threadIdx.x != 0) return;
   double ce = 0;
   for (int b = 0; b < B; ++b) ce += stats[b * K + C * kStat];
-  ce /= static_cast<double>(B) * static_cast<double>(plane);
+  if constexpr (IGN) {
+    double valid = 0;
+    for (int b = 0; b < B; ++b) valid += stats[b * K + C * kStat + 1];
+    ce = valid > 0 ? ce / valid : 0.0;  // no valid pixel: the reference skips the CE (compound_losses.py:52-53)
+  } else {
+    ce /= static_cast<double>(B) * static_cast<double>(plane);
+  }
   const int c0 = do_bg ? 0 : 1;
   double dc = 0;
   if (batch_dice) {
@@ -200,18 +217,24 @@ __global__ void loss_finalize_kernel(const double* __restrict__ partial, double*
       }
 }
 
-template <int C>
+// IGN: the CE weight is w_ce / (valid pixels of the batch), 0 without any, and the gradient is 0 at ignored pixels.
+template <int C, bool IGN = false>
 __global__ void __launch_bounds__(256) loss_grad_kernel(const float* __restrict__ logits, const void* __restrict__ target,
                                                         int tkind, const double* __restrict__ stats,
                                                         const double* __restrict__ gsum, float* __restrict__ grad,
                                                         int B, long long plane, float w_ce, float w_dice, int batch_dice,
                                                         int do_bg, float smooth, float grad_scale,
                                                         const float* __restrict__ ce_scale,
-                                                        const float* __restrict__ dice_scale) {
+                                                        const float* __restrict__ dice_scale, int ignore_label) {
   const int b = blockIdx.y;
-  constexpr int K = C * kStat + 1;
+  constexpr int K = C * kStat + 1 + IGN;
   // per-class dice coefficients a_c, b_c with d(dice term)/dp_c = a_c * y_c + b_c
-  __shared__ float sa[C], sb[C];
+  __shared__ float sa[C], sb[C], s_ce;
+  if (IGN && threadIdx.x == 32) {
+    double valid = 0;
+    for (int n = 0; n < B; ++n) valid += stats[n * K + C * kStat + 1];
+    s_ce = valid > 0 ? static_cast<float>(w_ce / valid) * (ce_scale ? *ce_scale : 1.f) : 0.f;
+  }
   if (threadIdx.x < C) {
     const int c = threadIdx.x, c0 = do_bg ? 0 : 1;
     float a = 0.f, bb = 0.f;
@@ -240,13 +263,21 @@ __global__ void __launch_bounds__(256) loss_grad_kernel(const float* __restrict_
   __syncthreads();
   const float* zb = logits + static_cast<long long>(b) * C * plane;
   float* gb = grad + static_cast<long long>(b) * C * plane;
-  const float ce_w = w_ce / (static_cast<float>(B) * static_cast<float>(plane)) * (ce_scale ? *ce_scale : 1.f);
+  const float ce_w = IGN ? s_ce
+                         : w_ce / (static_cast<float>(B) * static_cast<float>(plane)) * (ce_scale ? *ce_scale : 1.f);
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < plane;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     float p[C], mx, lse;
     int amax;
     pixel_softmax<C>(zb + i, plane, p, mx, lse, amax);
     int t = label_at(target, tkind, static_cast<long long>(b) * plane + i);
+    if constexpr (IGN) {
+      if (t == ignore_label) {
+#pragma unroll
+        for (int c = 0; c < C; ++c) gb[c * plane + i] = 0.f;
+        continue;
+      }
+    }
     if (t < 0 || t >= C) t = 0;
     float g[C], dot = 0.f;
 #pragma unroll
@@ -416,6 +447,10 @@ extern "C" int64_t b2u_dice_ce_work_doubles(int32_t B, int32_t C, int64_t plane)
   return static_cast<int64_t>(B) * stats_blocks(plane) * (C * kStat + 1) + static_cast<int64_t>(B) * (C * kStat + 1);
 }
 
+extern "C" int64_t b2u_dice_ce_ign_work_doubles(int32_t B, int32_t C, int64_t plane) {
+  return static_cast<int64_t>(B) * stats_blocks(plane) * (C * kStat + 2) + static_cast<int64_t>(B) * (C * kStat + 2);
+}
+
 extern "C" int64_t b2u_dice_bce_work_doubles(int32_t B, int32_t R, int64_t plane) {
   const int64_t K = R * kStat + kRegionExtra;
   return static_cast<int64_t>(B) * stats_blocks(plane) * K + static_cast<int64_t>(B) * K;
@@ -468,12 +503,14 @@ extern "C" int64_t b2u_dice_bce_work_doubles(int32_t B, int32_t R, int64_t plane
     B2U_LOSS_SWITCH(R, BODY)          \
   }
 
+template <bool IGN = false>
 static int dice_ce_stats(const float* logits, const void* target, int32_t target_kind, double* work,
-                         int32_t* bad_label, int32_t B, int32_t C, int64_t plane, cudaStream_t stream) {
+                         int32_t* bad_label, int32_t B, int32_t C, int64_t plane, cudaStream_t stream,
+                         int32_t ignore_label = 0) {
   const int nblk = stats_blocks(plane);
   dim3 grid(nblk, B);
-  B2U_LOSS_SWITCH(C, (loss_stats_kernel<CC><<<grid, 256, 0, stream>>>(logits, target, target_kind, work, bad_label,
-                                                                      plane));)
+  B2U_LOSS_SWITCH(C, (loss_stats_kernel<CC, IGN><<<grid, 256, 0, stream>>>(logits, target, target_kind, work,
+                                                                           bad_label, plane, ignore_label));)
   return check_launch("dice_ce_stats");
 }
 
@@ -500,7 +537,9 @@ extern "C" int b2u_dice_ce_stats(const float* logits, const void* target, int32_
   if (!logits || !target || !work || !batch_sums || !bad_label) return set_error(-1, "b2u_dice_ce_stats: null pointer");
   if (B <= 0 || plane <= 0 || target_kind < 0 || target_kind > 3) return set_error(-1, "b2u_dice_ce_stats: bad argument");
   if (int rc = dice_ce_stats(logits, target, target_kind, work, bad_label, B, C, plane, stream)) return rc;
-  dice_batch_sums_kernel<<<1, 128, 0, stream>>>(work, batch_sums, B, C, C * kStat + 1, stats_blocks(plane));
+  const int nblk = stats_blocks(plane), K = C * kStat + 1;
+  dice_batch_sums_kernel<<<1, 256, 0, stream>>>(work, work + static_cast<int64_t>(B) * nblk * K, batch_sums, B, C, K,
+                                                nblk);
   return check_launch("dice_ce_batch_sums");
 }
 
@@ -517,19 +556,22 @@ extern "C" int b2u_dice_ce_finalize(double* work, const double* batch_sums, floa
   return check_launch("dice_ce_finalize");
 }
 
+template <bool IGN = false>
 static int dice_ce_grad(const float* logits, const void* target, int32_t target_kind, const double* work,
                         const double* batch_sums, float* grad_logits, int32_t B, int32_t C, int64_t plane,
                         float weight_ce, float weight_dice, int32_t batch_dice, int32_t do_bg, float smooth,
-                        float grad_scale, const float* ce_scale, const float* dice_scale, cudaStream_t stream) {
+                        float grad_scale, const float* ce_scale, const float* dice_scale, cudaStream_t stream,
+                        int32_t ignore_label = 0) {
   if (!logits || !target || !work || !grad_logits) return set_error(-1, "b2u_dice_ce_backward: null pointer");
   if (target_kind < 0 || target_kind > 3) return set_error(-1, "b2u_dice_ce_backward: bad target kind");
   const int nblk = stats_blocks(plane);
-  const double* stats = work + static_cast<int64_t>(B) * nblk * (C * kStat + 1);
+  const double* stats = work + static_cast<int64_t>(B) * nblk * (C * kStat + 1 + IGN);
   dim3 grid(grad_blocks(plane), B);
-  B2U_LOSS_SWITCH(C, (loss_grad_kernel<CC><<<grid, 256, 0, stream>>>(logits, target, target_kind, stats, batch_sums,
-                                                                     grad_logits, B, plane, weight_ce, weight_dice,
-                                                                     batch_dice, do_bg, smooth, grad_scale, ce_scale,
-                                                                     dice_scale));)
+  B2U_LOSS_SWITCH(C, (loss_grad_kernel<CC, IGN><<<grid, 256, 0, stream>>>(logits, target, target_kind, stats,
+                                                                          batch_sums, grad_logits, B, plane, weight_ce,
+                                                                          weight_dice, batch_dice, do_bg, smooth,
+                                                                          grad_scale, ce_scale, dice_scale,
+                                                                          ignore_label));)
   return check_launch("dice_ce_backward");
 }
 
@@ -551,6 +593,49 @@ extern "C" int b2u_dice_ce_backward_scaled(const float* logits, const void* targ
                       batch_dice, do_bg, smooth, 1.f, ce_scale, dice_scale, static_cast<cudaStream_t>(stream_));
 }
 
+// ---- the same loss with an ignore label (label maps of sparsely annotated datasets): split forward as above, the
+// per-sample records carry the valid-pixel count, the backward takes its scales from the device.
+extern "C" int b2u_dice_ce_ign_stats(const float* logits, const void* target, int32_t target_kind, int32_t ignore_label,
+                                     double* work, double* batch_sums, int32_t* bad_label, int32_t B, int32_t C,
+                                     int64_t plane, b2u_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (!logits || !target || !work || !batch_sums || !bad_label)
+    return set_error(-1, "b2u_dice_ce_ign_stats: null pointer");
+  if (B <= 0 || plane <= 0 || target_kind < 0 || target_kind > 3)
+    return set_error(-1, "b2u_dice_ce_ign_stats: bad argument");
+  if (int rc = dice_ce_stats<true>(logits, target, target_kind, work, bad_label, B, C, plane, stream, ignore_label))
+    return rc;
+  const int nblk = stats_blocks(plane), K = C * kStat + 2;
+  dice_batch_sums_kernel<<<1, 256, 0, stream>>>(work, work + static_cast<int64_t>(B) * nblk * K, batch_sums, B, C, K,
+                                                nblk);
+  return check_launch("dice_ce_ign_batch_sums");
+}
+
+extern "C" int b2u_dice_ce_ign_finalize(double* work, const double* batch_sums, float* out3, int64_t* tp_fp_fn,
+                                        int32_t B, int32_t C, int64_t plane, float weight_ce, float weight_dice,
+                                        int32_t batch_dice, int32_t do_bg, float smooth, b2u_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (!work || !batch_sums || !out3) return set_error(-1, "b2u_dice_ce_ign_finalize: null pointer");
+  if (B <= 0 || plane <= 0 || C < 2 || C > 32) return set_error(-1, "b2u_dice_ce_ign_finalize: bad argument");
+  const int nblk = stats_blocks(plane);
+  double* stats = work + static_cast<int64_t>(B) * nblk * (C * kStat + 2);
+  loss_finalize_kernel<true><<<1, 256, 0, stream>>>(work, stats, batch_sums, out3, tp_fp_fn, B, C, nblk, plane,
+                                                    weight_ce, weight_dice, batch_dice, do_bg, smooth);
+  return check_launch("dice_ce_ign_finalize");
+}
+
+extern "C" int b2u_dice_ce_ign_backward(const float* logits, const void* target, int32_t target_kind,
+                                        int32_t ignore_label, const double* work, const double* batch_sums,
+                                        float* grad_logits, int32_t B, int32_t C, int64_t plane, float weight_ce,
+                                        float weight_dice, int32_t batch_dice, int32_t do_bg, float smooth,
+                                        const float* ce_scale, const float* dice_scale, b2u_stream_t stream_) {
+  if (!batch_sums || !ce_scale || !dice_scale) return set_error(-1, "b2u_dice_ce_ign_backward: null pointer");
+  if (B <= 0 || plane <= 0) return set_error(-1, "b2u_dice_ce_ign_backward: bad argument");
+  return dice_ce_grad<true>(logits, target, target_kind, work, batch_sums, grad_logits, B, C, plane, weight_ce,
+                            weight_dice, batch_dice, do_bg, smooth, 1.f, ce_scale, dice_scale,
+                            static_cast<cudaStream_t>(stream_), ignore_label);
+}
+
 static int region_args(const char* fn, const float* logits, const void* target, int32_t target_kind, int32_t B,
                        int32_t R, int64_t plane) {
   if (!logits || !target) return set_error(-1, "%s: null pointer", fn);
@@ -570,7 +655,9 @@ extern "C" int b2u_dice_bce_stats(const float* logits, const void* target, int32
   B2U_REGION_SWITCH(R, (region_stats_kernel<CC><<<grid, 256, 0, stream>>>(logits, target, target_kind, ign, work,
                                                                           plane));)
   if (int rc = check_launch("dice_bce_stats")) return rc;
-  dice_batch_sums_kernel<<<1, 128, 0, stream>>>(work, batch_sums, B, R, R * kStat + kRegionExtra, nblk);
+  const int K = R * kStat + kRegionExtra;
+  dice_batch_sums_kernel<<<1, 256, 0, stream>>>(work, work + static_cast<int64_t>(B) * nblk * K, batch_sums, B, R, K,
+                                                nblk);
   return check_launch("dice_bce_batch_sums");
 }
 

@@ -15,7 +15,14 @@ the finalisation, as the reference's AllGatherGrad + sum does (dice.py:106-110).
 plus the global Dice term; in backward the Dice part of the gradient is scaled by the sum of the ranks' incoming
 gradients (the AllGatherGrad backward, ddp_allgather.py:43-48).  Both happen on the current stream, without a host sync.
 
-Not covered (raise): the ignore label of the softmax loss.
+Ignore label of the softmax loss (`DC_and_CE_loss(..., ignore_label=N)`, sparsely annotated label maps): pixels labelled N
+add nothing to the Dice sums, the CE (mean over the valid pixels of the local batch, 0 when there are none, as the
+reference skips it) or the validation counts, and their gradient is exactly 0.  It runs the split entry points
+(b2u_dice_ce_ign_*), with the same data-parallel batch Dice; the CE weight 1 / #valid stays on the device.
+
+Not covered (raise): an ignore label with `do_bg=True`.  The ignore-label loss covers the configuration the reference
+trainer builds for label maps (Dice without the background class, nnUNetTrainer.py:363-365), as the region loss covers
+only its trainer configuration (do_bg=True).
 """
 from typing import Dict
 
@@ -137,6 +144,52 @@ class _DiceCEAllReduced(Function):
         return grad.view(ctx.in_shape).to(ctx.in_dtype), None, None, None, None, None
 
 
+class _DiceCEIgnore(Function):
+    """Dice + CE over the pixels whose label is not `ignore_label` (compound_losses.py:38-53); the batch Dice sums are
+    all-reduced across the data-parallel ranks when `all_reduce`."""
+
+    @staticmethod
+    def forward(ctx, logits, target, ignore_label, weight_ce, weight_dice, batch_dice, do_bg, smooth, all_reduce):
+        z, t, B, C, plane = _prep(logits, target)
+        lib = L.load()
+        dev = z.device
+        work = torch.empty(int(lib.b2u_dice_ce_ign_work_doubles(B, C, plane)), dtype=torch.float64, device=dev)
+        bsum = torch.empty((C, 3), dtype=torch.float64, device=dev)
+        out3 = torch.empty(3, dtype=torch.float32, device=dev)
+        counts = torch.empty((3, C), dtype=torch.int64, device=dev)
+        bad = torch.zeros(1, dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            L.check(lib.b2u_dice_ce_ign_stats(z.data_ptr(), t.data_ptr(), _KIND[t.dtype], ignore_label, work.data_ptr(),
+                                              bsum.data_ptr(), bad.data_ptr(), B, C, plane,
+                                              torch.cuda.current_stream(dev).cuda_stream), "dice_ce_ign_stats")
+            if all_reduce:
+                torch.distributed.all_reduce(bsum)
+            L.check(lib.b2u_dice_ce_ign_finalize(work.data_ptr(), bsum.data_ptr(), out3.data_ptr(), counts.data_ptr(), B,
+                                                 C, plane, float(weight_ce), float(weight_dice), int(batch_dice),
+                                                 int(do_bg), float(smooth), torch.cuda.current_stream(dev).cuda_stream),
+                    "dice_ce_ign_finalize")
+        ctx.save_for_backward(z, t, work, bsum)
+        ctx.cfg = (ignore_label, B, C, plane, float(weight_ce), float(weight_dice), int(batch_dice), int(do_bg),
+                   float(smooth), bool(all_reduce))
+        ctx.in_dtype, ctx.in_shape = logits.dtype, logits.shape
+        ctx.mark_non_differentiable(out3, counts, bad)
+        return out3[0].clone(), out3, counts, bad
+
+    @staticmethod
+    def backward(ctx, g, *_unused):
+        z, t, work, bsum = ctx.saved_tensors
+        ign, B, C, plane, wce, wdc, bd, bg, smooth, all_reduce = ctx.cfg
+        local, total = _grad_scales(g, all_reduce)
+        grad = torch.empty_like(z)
+        with torch.cuda.device(z.device):
+            L.check(L.load().b2u_dice_ce_ign_backward(z.data_ptr(), t.data_ptr(), _KIND[t.dtype], ign, work.data_ptr(),
+                                                      bsum.data_ptr(), grad.data_ptr(), B, C, plane, wce, wdc, bd, bg,
+                                                      smooth, local.data_ptr(), total.data_ptr(),
+                                                      torch.cuda.current_stream(z.device).cuda_stream),
+                    "dice_ce_ign_backward")
+        return grad.view(ctx.in_shape).to(ctx.in_dtype), None, None, None, None, None, None, None, None
+
+
 def _prep_regions(logits: torch.Tensor, target: torch.Tensor, has_ignore: bool):
     if not logits.is_cuda:
         raise L.NativeLibraryError("dinounet_b200 losses run on CUDA tensors only (no CPU fallback)")
@@ -200,7 +253,9 @@ class DC_and_CE_loss(nn.Module):
                  dice_class=None):
         super().__init__()
         if ignore_label is not None:
-            raise NotImplementedError("ignore_label is not covered by the fused native loss")
+            if int(ignore_label) != ignore_label or not -2 ** 31 <= int(ignore_label) < 2 ** 31:
+                raise ValueError(f"ignore_label must be a 32-bit integer, got {ignore_label!r}")
+            ignore_label = int(ignore_label)
         if ce_kwargs:
             raise NotImplementedError(f"cross-entropy options {sorted(ce_kwargs)} are not covered by the fused native loss")
         kw = dict(soft_dice_kwargs)
@@ -211,13 +266,21 @@ class DC_and_CE_loss(nn.Module):
         kw.pop("apply_nonlin", None)
         if kw:
             raise NotImplementedError(f"soft dice options {sorted(kw)} are not covered by the fused native loss")
+        if ignore_label is not None and self.do_bg:
+            raise NotImplementedError("ignore_label with do_bg=True is not covered by the fused native loss (the "
+                                      "trainer's label-map loss, do_bg=False, is)")
         self.weight_dice = weight_dice
         self.weight_ce = weight_ce
-        self.ignore_label = None
-        self.check_labels = False     # True: synchronise and raise on labels outside [0, C) (torch device-asserts)
+        self.ignore_label = ignore_label
+        # True: synchronise and raise on labels outside [0, C) other than ignore_label (torch device-asserts)
+        self.check_labels = False
 
     def _run(self, net_output, target):
-        if _ddp_batch_dice(self.batch_dice, self.ddp):
+        if self.ignore_label is not None:
+            loss, out3, counts, bad = _DiceCEIgnore.apply(net_output, target, self.ignore_label, self.weight_ce,
+                                                          self.weight_dice, self.batch_dice, self.do_bg, self.smooth,
+                                                          _ddp_batch_dice(self.batch_dice, self.ddp))
+        elif _ddp_batch_dice(self.batch_dice, self.ddp):
             loss, out3, counts, bad = _DiceCEAllReduced.apply(net_output, target, self.weight_ce, self.weight_dice,
                                                               self.do_bg, self.smooth)
         else:
@@ -266,8 +329,8 @@ class DC_and_BCE_loss(nn.Module):
 
 def validation_statistics(loss_module, net_output: torch.Tensor, target: torch.Tensor) -> Dict[str, np.ndarray]:
     """What `nnUNetTrainer.validation_step` returns for one batch (nnUNetTrainer.py:961-1005): the loss and the hard
-    tp / fp / fn, float32.  Label maps (`DC_and_CE_loss`): argmax(net_output) per foreground class (background dropped).
-    Regions (`DC_and_BCE_loss`): sigmoid(net_output) > 0.5 per region, each pixel weighted by 1 - t_ign when the target
+    tp / fp / fn, float32.  Label maps (`DC_and_CE_loss`): argmax(net_output) per foreground class (background dropped),
+    over the pixels not labelled with the loss's ignore label.  Regions (`DC_and_BCE_loss`): sigmoid(net_output) > 0.5 per region, each pixel weighted by 1 - t_ign when the target
     carries an ignore channel.  Under data-parallel batch Dice the loss uses the all-reduced sums; the counts stay per
     rank (the trainer gathers them at the end of the epoch)."""
     with torch.no_grad():

@@ -218,7 +218,7 @@ int b2u_sw_finalize(void* acc, const void* npred, int32_t C, int64_t plane, int3
  *   batch (get_tp_fp_fn_tn with axes (0,2,3), nnUNetTrainer.py:971-991);  *bad_label is set to 1 if a label is outside
  *   [0, C) (torch raises a device assert there).  Deterministic (fixed reduction order, fp64 partials).
  * backward: grad_logits fp32 [B, C, plane] = grad_scale * dLoss/dlogits, from the sums the forward left in `work`.
- * 2 <= C <= 32.  ignore_label is not covered.
+ * 2 <= C <= 32.  An ignore label takes the b2u_dice_ce_ign_* family below.
  *
  * Split forward for data-parallel batch Dice (dice.py:106-110, AllGatherGrad): b2u_dice_ce_stats runs the statistics
  * pass and writes batch_sums fp64 [C][3] = (intersect, sum_pred, sum_gt) of every class summed over the local batch;
@@ -242,6 +242,29 @@ int b2u_dice_ce_backward_scaled(const float* logits, const void* target, int32_t
                                 const double* batch_sums, float* grad_logits, int32_t B, int32_t C, int64_t plane,
                                 float weight_ce, float weight_dice, int32_t batch_dice, int32_t do_bg, float smooth,
                                 const float* ce_scale, const float* dice_scale, b2u_stream_t stream);
+
+/* ---- The same loss with an ignore label (DC_and_CE_loss(..., ignore_label), compound_losses.py:21-22, 38-53;
+ * validation_step's label-map mask, nnUNetTrainer.py:982-986).  A pixel whose label equals ignore_label (any integer;
+ * nnU-Net uses C) is ignored; the others are valid.  work: b2u_dice_ce_ign_work_doubles(B, C, plane) doubles; the
+ * per-sample records also hold the valid-pixel count.
+ * stats: one pass; batch_sums fp64 [C][3] = (intersect, sum_pred, sum_gt) over the valid pixels, summed over the batch
+ *   (all-reducible as above); *bad_label = 1 if a valid pixel's label is outside [0, C).
+ * finalize: out3[1] = CE summed over the valid pixels / their number (0 when the batch has none: the reference skips
+ *   the CE), out3[2] = the dice term over the valid pixels (batch Dice from batch_sums when batch_dice), out3[0] =
+ *   weight_ce*CE + weight_dice*dice;  tp_fp_fn (optional) int64 [3][C] = hard counts over the valid pixels only.
+ * backward: grad = *ce_scale * dCE/dlogits + *dice_scale * d(dice term)/dlogits, exactly 0 at ignored pixels; the CE
+ *   weight weight_ce / #valid is formed on the device.  Deterministic (fixed reduction order, fp64 partials). */
+int64_t b2u_dice_ce_ign_work_doubles(int32_t B, int32_t C, int64_t plane);
+int b2u_dice_ce_ign_stats(const float* logits, const void* target, int32_t target_kind, int32_t ignore_label,
+                          double* work, double* batch_sums, int32_t* bad_label, int32_t B, int32_t C, int64_t plane,
+                          b2u_stream_t stream);
+int b2u_dice_ce_ign_finalize(double* work, const double* batch_sums, float* out3, int64_t* tp_fp_fn, int32_t B,
+                             int32_t C, int64_t plane, float weight_ce, float weight_dice, int32_t batch_dice,
+                             int32_t do_bg, float smooth, b2u_stream_t stream);
+int b2u_dice_ce_ign_backward(const float* logits, const void* target, int32_t target_kind, int32_t ignore_label,
+                             const double* work, const double* batch_sums, float* grad_logits, int32_t B, int32_t C,
+                             int64_t plane, float weight_ce, float weight_dice, int32_t batch_dice, int32_t do_bg,
+                             float smooth, const float* ce_scale, const float* dice_scale, b2u_stream_t stream);
 
 /* ---- Region-based Dice + BCE (compound_losses.py:59-99 `DC_and_BCE_loss` with MemoryEfficientSoftDiceLoss on
  * sigmoid(logits), do_bg, built at nnUNetTrainer.py:356-361; validation_step's region branch :973-994).

@@ -18,6 +18,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from dinounet_b200.loss import DC_and_BCE_loss, DC_and_CE_loss  # noqa: E402
+from oracle import ignore_loss_oracle as IO  # noqa: E402
 from oracle import loss_oracle as LO  # noqa: E402
 from oracle import region_loss_oracle as RO  # noqa: E402
 
@@ -70,6 +71,11 @@ def main():
     t = torch.randint(0, 2, (B, 1, S, S), generator=g).float().to(dev)
     ce = DC_and_CE_loss({"batch_dice": True, "smooth": 1e-5, "do_bg": False, "ddp": False}, {}, 1, 1)
     configs.append(("softmax C=2", z, t, ce, lambda zz, tt: LO.dc_and_ce_loss(zz, tt)[0], 2 * (2 * 4 + 4) + 2 * 4))
+    z, t = IO.ignore_case(B, 2, S, S, 2)          # about 20 % of the pixels labelled 2, the ignore label
+    z, t = z.to(dev), t.to(dev)
+    ce = DC_and_CE_loss({"batch_dice": True, "smooth": 1e-5, "do_bg": False, "ddp": False}, {}, 1, 1, ignore_label=2)
+    configs.append(("softmax C=2, ignore label", z, t, ce, lambda zz, tt: IO.dc_and_ce_loss(zz, tt, 2)[0],
+                    2 * (2 * 4 + 4) + 2 * 4))
     for ign in (False, True):
         z, t = RO.region_case(B, 3, S, S, 1, use_ignore=ign)
         z, t = z.to(dev), t.to(dev)
