@@ -94,6 +94,8 @@ SIGNATURES = {
     "b2u_sw_gather_tiles": [vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp],
     "b2u_sw_accumulate": [vp, vp, i32, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp],
     "b2u_sw_finalize": [vp, vp, i32, i64, vp, vp],
+    "b2u_export_resample_f16": [vp, vp, i32, i32, i32, i32, i32, i32, vp],
+    "b2u_export_segment": [vp, i32, i64, i32, vp, vp, i32, vp, vp],
     "b2u_dice_ce_work_doubles": [i32, i32, i64],
     "b2u_dice_ce_forward": [vp, vp, i32, vp, vp, vp, vp, i32, i32, i64, f32, f32, i32, i32, f32, vp],
     "b2u_dice_ce_backward": [vp, vp, i32, vp, vp, i32, i32, i64, f32, f32, i32, i32, f32, f32, vp],

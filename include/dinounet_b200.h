@@ -207,6 +207,21 @@ int b2u_sw_accumulate(const float* logits, const int32_t* tile_desc, int32_t fir
                       b2u_stream_t stream);
 int b2u_sw_finalize(void* acc, const void* npred, int32_t C, int64_t plane, int32_t* inf_flag, b2u_stream_t stream);
 
+/* ---- Prediction export (inference/export_prediction.py:15-68), the two device steps before the host paste.
+ * b2u_export_resample_f16: fp16 [C, Z, h, w] -> fp16 [C, Z, H, W], Z unchanged: the 2D configuration's
+ *   `resampling_fn_probabilities` (resample_data_or_seg_to_shape, order 1; default_resampling.py), i.e. scipy
+ *   ndimage.zoom(order=1, mode='nearest', grid_mode=True) in fp64 with scipy's exact coordinate and weight arithmetic,
+ *   rounded to fp16 to nearest even.  Bit-identical to the reference for finite logits; h == H && w == W copies `in`
+ *   (the reference returns the array unchanged).  `in` and `out` must not overlap otherwise.
+ * b2u_export_segment: fp16 logits [C, voxels], 1 <= C <= 32.  mode 0 (label maps): fp32 softmax over C, labels = index
+ *   of the first maximum probability.  mode 1 (regions): fp32 sigmoid, labels = region_labels[i] (DEVICE int32 [C]) of
+ *   the last channel i with p > 0.5, else 0 (label_handling.py:128-175).  labels: uint8 (label_bytes 1) or uint16 (2)
+ *   [voxels]; probs: fp32 [C, voxels], written only when non-NULL.  No atomics: repeated launches give identical bits. */
+int b2u_export_resample_f16(const void* in, void* out, int32_t C, int32_t Z, int32_t h, int32_t w, int32_t H, int32_t W,
+                            b2u_stream_t stream);
+int b2u_export_segment(const void* logits, int32_t C, int64_t voxels, int32_t mode, const int32_t* region_labels,
+                       void* labels, int32_t label_bytes, float* probs, b2u_stream_t stream);
+
 /* ---- Dice + cross-entropy loss and online-validation statistics on the logits of the forward path
  * (training/loss/compound_losses.py:31-56 `DC_and_CE_loss`, dice.py:72-119 `MemoryEfficientSoftDiceLoss`,
  * robust_ce_loss.py:12-16, built at nnUNetTrainer.py:363-365; consumer nnUNetTrainer.py:961-1005 `validation_step`).
