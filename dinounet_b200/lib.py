@@ -96,6 +96,12 @@ SIGNATURES = {
     "b2u_sw_finalize": [vp, vp, i32, i64, vp, vp],
     "b2u_export_resample_f16": [vp, vp, i32, i32, i32, i32, i32, i32, vp],
     "b2u_export_segment": [vp, i32, i64, i32, vp, vp, i32, vp, vp],
+    "b2u_pre_minmax_f32": [vp, i64, vp, vp, vp, vp],
+    "b2u_pre_zscore": [vp, i64, i32, i32, i32, i64, i64, i64, vp, vp, vp],
+    "b2u_pre_normalize": [vp, i64, i32, vp, f32, f32, f32, f32, vp],
+    "b2u_pre_resample3_work_doubles": [i32, i32, i32, i32],
+    "b2u_pre_resample3": [vp, i32, i32, i32, i64, i64, i64, i32, i32, i32, vp, vp, vp, vp],
+    "b2u_pre_ensemble_f16": [vp, vp, i64, i32, vp],
     "b2u_dice_ce_work_doubles": [i32, i32, i64],
     "b2u_dice_ce_forward": [vp, vp, i32, vp, vp, vp, vp, i32, i32, i64, f32, f32, i32, i32, f32, vp],
     "b2u_dice_ce_backward": [vp, vp, i32, vp, vp, i32, i32, i64, f32, f32, i32, i32, f32, f32, vp],
@@ -168,7 +174,7 @@ SIGNATURES = {
 _RESTYPES = {"b2u_last_error": C.c_char_p, "b2u_launch_count": C.c_int64, "b2u_in_stats_work_floats": C.c_int64,
              "b2u_dice_ce_work_doubles": C.c_int64, "b2u_dice_ce_ign_work_doubles": C.c_int64,
              "b2u_dice_bce_work_doubles": C.c_int64,
-             "b2u_f32_bn_work_doubles": C.c_int64}
+             "b2u_f32_bn_work_doubles": C.c_int64, "b2u_pre_resample3_work_doubles": C.c_int64}
 
 _lib: Optional[C.CDLL] = None
 

@@ -221,3 +221,55 @@ class SlidingWindowPredictor:
                                "predicted_logits to fp32")
         out = acc[(slice(None), *revert[1:])]
         return out if self.perform_everything_on_device else out.cpu()
+
+    @torch.no_grad()
+    def predict_logits_from_preprocessed_data(self, data: torch.Tensor) -> torch.Tensor:
+        """predict_from_raw_data.py:466-501: the sliding window once per entry of `list_of_parameters` (loaded into the
+        network), summed and divided by the number of folds in fp16 with the bits of the reference's CPU fp16 ops
+        (`b2u_pre_ensemble_f16`).  The fp16 logits [heads, *data.shape[1:]] stay on the device.  With
+        `list_of_parameters` None the network's current weights make the single prediction."""
+        from .preprocess import ensemble_logits
+        lib = L.load()
+        params = self.list_of_parameters
+
+        def runs():
+            for p in (params or [None]):
+                if p is not None:
+                    self.network.load_state_dict(p)
+                    if hasattr(self.network, "repack"):
+                        self.network.repack()   # the engine packs the weights it was built with
+                logits = self.predict_sliding_window_return_logits(data)
+                yield logits if logits.is_cuda else logits.to(self.device)
+
+        def add(acc, x, divisor):
+            with torch.cuda.device(acc.device):
+                L.check(lib.b2u_pre_ensemble_f16(acc.data_ptr(), None if x is None else x.data_ptr(), acc.numel(),
+                                                 divisor, torch.cuda.current_stream(acc.device).cuda_stream),
+                        "b2u_pre_ensemble_f16")
+
+        return ensemble_logits(runs(), len(params) if params else 1, add)
+
+    def predict_single_npy_array(self, input_image: np.ndarray, image_properties: dict,
+                                 segmentation_previous_stage: np.ndarray = None, output_file_truncated: str = None,
+                                 save_or_return_probabilities: bool = False):
+        """predict_from_raw_data.py:429-464 on the device: DevicePreprocessor.run_case_npy -> the fold ensemble ->
+        the device export.  Only the input goes up, and only the segmentation (and the probabilities, when asked) comes
+        down.  `image_properties` needs the 'spacing' key; the preprocessing adds its keys to it, as the reference's."""
+        from . import export
+        from .preprocess import DevicePreprocessor
+        if segmentation_previous_stage is not None:
+            raise NotImplementedError("the cascade (segmentation_previous_stage) is not implemented on the device")
+        if self.plans_manager is None:
+            raise ValueError("predict_single_npy_array needs a plans_manager (manual_initialization)")
+        dev = self.device if self.device.index is not None else torch.device("cuda", torch.cuda.current_device())
+        data, _ = DevicePreprocessor(self.verbose_preprocessing, dev).run_case_npy(
+            input_image, None, image_properties, self.plans_manager, self.configuration_manager, self.dataset_json)
+        logits = self.predict_logits_from_preprocessed_data(data)
+        if output_file_truncated is not None:
+            export.export_prediction_from_logits(logits, image_properties, self.configuration_manager,
+                                                 self.plans_manager, self.dataset_json, output_file_truncated,
+                                                 save_or_return_probabilities)
+            return None
+        return export.convert_predicted_logits_to_segmentation_with_correct_shape(
+            logits, self.plans_manager, self.configuration_manager, self.label_manager, image_properties,
+            return_probabilities=save_or_return_probabilities)

@@ -222,6 +222,35 @@ int b2u_export_resample_f16(const void* in, void* out, int32_t C, int32_t Z, int
 int b2u_export_segment(const void* logits, int32_t C, int64_t voxels, int32_t mode, const int32_t* region_labels,
                        void* labels, int32_t label_bytes, float* probs, b2u_stream_t stream);
 
+/* ---- Case preprocessing (preprocessing/preprocessors/default_preprocessor.py:40-118 `run_case_npy` of a 2D
+ * configuration), fp32 channels in the caller's memory.  Bit-identical to numpy / scipy for finite input.
+ * b2u_pre_minmax_f32: lo_hi[0..1] = exact min / max of x[n]; *nonfinite = 1 if x holds a NaN or an infinity (left
+ *   untouched otherwise; may be NULL).  work: 2 * ceil(n / 65536) floats.
+ * b2u_pre_zscore: ZScoreNormalization (default_normalization_schemes.py:27-50) in place on x[n]: numpy's float32 mean and
+ *   std as ONE pairwise sum (numpy's pairwise_sum tree) over the elements in the order (i0, i1, i2) -> x[i0*s0 + i1*s1 +
+ *   i2*s2], n = n0*n1*n2 (memory order: 1, 1, n, 0, 0, 1; use_mask_for_norm gathers in the transposed view's order);
+ *   stats[0] = mean, stats[1] = max(std, 1e-8f), both left on the device.  work: ceil(n / 8) floats.
+ * b2u_pre_normalize: scheme 1 CTNormalization x = (clip(x, a, b) - c) / d; 2 RescaleTo01 x = (x - stats[0]) /
+ *   max(stats[1] - stats[0], 1e-8f) with stats the device [min, max] of x; 3 RGBTo01 x = x / 255.
+ * b2u_pre_resample3: resample_data_or_seg_to_shape(order=3) of one channel (default_resampling.py:77-216), Z unchanged:
+ *   x is the normalized channel as a [Z, h, w] view (element strides sz, sy, sx: the transpose is folded into the read),
+ *   out fp32 [Z, H, W] contiguous.  three_d 0: separate z along axis 0, a 2-D resize per slice; 1: one 3-D resize.  Each
+ *   is skimage resize(order=3, mode='edge') = scipy ndimage.zoom(order=3, mode='nearest', grid_mode=True) in fp64 with
+ *   scipy's arithmetic, clipped to the slice's (0) or channel's (1) [min, max], rounded once to fp32.  consts: HOST
+ *   array of 15 doubles, per axis (z, y, x) {pole, pole^n, gain, pole / (1 - pole^2n), pole / (pole - 1)} with n the
+ *   padded length (Z + 24 or unused, h + 24, w + 24).  work: b2u_pre_resample3_work_doubles(Z, h, w, three_d) doubles.
+ * b2u_pre_ensemble_f16: fold ensemble in fp16 as torch's CPU ops: acc = fp16(fp32(acc) + fp32(x)) when x != NULL, then
+ *   acc = fp16(fp32(acc) / divisor) when divisor > 0.  acc, x: fp16 [n]. */
+int b2u_pre_minmax_f32(const float* x, int64_t n, float* work, float* lo_hi, int32_t* nonfinite, b2u_stream_t stream);
+int b2u_pre_zscore(float* x, int64_t n, int32_t n0, int32_t n1, int32_t n2, int64_t s0, int64_t s1, int64_t s2,
+                   float* work, float* stats, b2u_stream_t stream);
+int b2u_pre_normalize(float* x, int64_t n, int32_t scheme, const float* stats, float a, float b, float c, float d,
+                      b2u_stream_t stream);
+int64_t b2u_pre_resample3_work_doubles(int32_t Z, int32_t h, int32_t w, int32_t three_d);
+int b2u_pre_resample3(const float* x, int32_t Z, int32_t h, int32_t w, int64_t sz, int64_t sy, int64_t sx, int32_t H,
+                      int32_t W, int32_t three_d, const double* consts, double* work, float* out, b2u_stream_t stream);
+int b2u_pre_ensemble_f16(void* acc, const void* x, int64_t n, int32_t divisor, b2u_stream_t stream);
+
 /* ---- Dice + cross-entropy loss and online-validation statistics on the logits of the forward path
  * (training/loss/compound_losses.py:31-56 `DC_and_CE_loss`, dice.py:72-119 `MemoryEfficientSoftDiceLoss`,
  * robust_ce_loss.py:12-16, built at nnUNetTrainer.py:363-365; consumer nnUNetTrainer.py:961-1005 `validation_step`).
