@@ -18,6 +18,10 @@ int encode_tensor_map(CUtensorMap* map, int dtype, int rank, const void* base, c
 
 int get_option(int key);
 
+// numpy's pairwise sum of a contiguous float64 x[n] (preprocess.cu's tree, shared with the float32 ZScore statistics):
+// the sum lands in work[0].  work: ceil(n / 8) doubles.
+int pairwise_sum_f64(const double* x, long long n, double* work, cudaStream_t stream);
+
 // Programmatic dependent launch (PDL), OPT-IN (option 5 = 1): every kernel of the forward plan can be launched with
 // cudaLaunchAttributeProgrammaticStreamSerialization; each calls `griddepcontrol.wait` before it touches global memory
 // (after its barrier-init / tensormap-prefetch prologue where it has one) and the persistent GEMM / attention

@@ -81,24 +81,33 @@ __global__ void __launch_bounds__(256) minmax_kernel(const T* __restrict__ lo_sr
   }
 }
 
-// ---- numpy's pairwise float32 sum ---------------------------------------------------------------------------------
+// ---- numpy's pairwise sum (float32 here, float64 for the evaluation's mean surface distance) ----------------------
 
 struct Order3 {  // element i of the summation order lives at i0*s0 + i1*s1 + i2*s2, i = (i0*n1 + i1)*n2 + i2
   long long n1, n2, s0, s1, s2;
   bool flat;     // s2 == 1 and the order is memory order
 };
 
-__device__ __forceinline__ float elem(const float* x, const Order3& o, long long i) {
+template <typename T>
+__device__ __forceinline__ T elem(const T* x, const Order3& o, long long i) {
   if (o.flat) return x[i];
   const long long i2 = i % o.n2, r = i / o.n2;
   return x[(r / o.n1) * o.s0 + (r % o.n1) * o.s1 + i2 * o.s2];
 }
 
-__device__ __forceinline__ float term(const float* x, const Order3& o, long long i, bool sq, float mean) {
-  const float v = elem(x, o, i);
+__device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
+__device__ __forceinline__ double add_rn(double a, double b) { return __dadd_rn(a, b); }
+__device__ __forceinline__ float sub_rn(float a, float b) { return __fsub_rn(a, b); }
+__device__ __forceinline__ double sub_rn(double a, double b) { return __dsub_rn(a, b); }
+__device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ double mul_rn(double a, double b) { return __dmul_rn(a, b); }
+
+template <typename T>
+__device__ __forceinline__ T term(const T* x, const Order3& o, long long i, bool sq, T mean) {
+  const T v = elem(x, o, i);
   if (!sq) return v;
-  const float d = __fsub_rn(v, mean);
-  return __fmul_rn(d, d);
+  const T d = sub_rn(v, mean);
+  return mul_rn(d, d);
 }
 
 __device__ __forceinline__ long long split_of(long long m) {
@@ -108,9 +117,9 @@ __device__ __forceinline__ long long split_of(long long m) {
 
 // One thread per node of depth k (path bits, root decision first).  A leaf (m <= 128) writes its sum to val[o / 8]; an
 // inner node adds its children, both already evaluated at depth k + 1, into the slot it shares with its left child.
-__global__ void __launch_bounds__(256) tree_level_kernel(const float* __restrict__ x, long long n, int k, Order3 ord,
-                                                         int sq, const float* __restrict__ stats,
-                                                         float* __restrict__ val) {
+template <typename T>
+__global__ void __launch_bounds__(256) tree_level_kernel(const T* __restrict__ x, long long n, int k, Order3 ord,
+                                                         int sq, const T* __restrict__ stats, T* __restrict__ val) {
   const long long b = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (b >= (1LL << k)) return;
   long long o = 0, m = n;
@@ -126,27 +135,26 @@ __global__ void __launch_bounds__(256) tree_level_kernel(const float* __restrict
   }
   if (m > kLeaf) {
     const long long m2 = split_of(m);
-    val[o / 8] = __fadd_rn(val[o / 8], val[(o + m2) / 8]);
+    val[o / 8] = add_rn(val[o / 8], val[(o + m2) / 8]);
     return;
   }
   const bool squares = sq != 0;
-  const float mean = squares ? stats[0] : 0.f;
-  float res;
+  const T mean = squares ? stats[0] : T(0);
+  T res;
   if (m < 8) {
-    res = 0.f;
-    for (long long i = 0; i < m; ++i) res = __fadd_rn(res, term(x, ord, o + i, squares, mean));
+    res = T(0);
+    for (long long i = 0; i < m; ++i) res = add_rn(res, term(x, ord, o + i, squares, mean));
   } else {
-    float r[8];
+    T r[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) r[j] = term(x, ord, o + j, squares, mean);
     long long i = 8;
     for (; i < m - m % 8; i += 8) {
 #pragma unroll
-      for (int j = 0; j < 8; ++j) r[j] = __fadd_rn(r[j], term(x, ord, o + i + j, squares, mean));
+      for (int j = 0; j < 8; ++j) r[j] = add_rn(r[j], term(x, ord, o + i + j, squares, mean));
     }
-    res = __fadd_rn(__fadd_rn(__fadd_rn(r[0], r[1]), __fadd_rn(r[2], r[3])),
-                    __fadd_rn(__fadd_rn(r[4], r[5]), __fadd_rn(r[6], r[7])));
-    for (; i < m; ++i) res = __fadd_rn(res, term(x, ord, o + i, squares, mean));
+    res = add_rn(add_rn(add_rn(r[0], r[1]), add_rn(r[2], r[3])), add_rn(add_rn(r[4], r[5]), add_rn(r[6], r[7])));
+    for (; i < m; ++i) res = add_rn(res, term(x, ord, o + i, squares, mean));
   }
   val[o / 8] = res;
 }
@@ -343,6 +351,26 @@ static int tree_depth(long long n) {
   }
 }
 
+// Evaluates the whole tree over x[n] (in the order `ord`; sq: sum of (x - stats[0])^2), deepest level first: the sum
+// lands in work[0].  work: ceil(n / 8) elements.
+template <typename T>
+static int pairwise_sum_tree(const T* x, long long n, const Order3& ord, int sq, const T* stats, T* work,
+                             cudaStream_t stream, const char* what) {
+  const int depth = tree_depth(n);
+  if (depth > 40) return set_error(-1, "%s: tree depth %d", what, depth);
+  for (int k = depth; k >= 0; --k) {
+    const long long nodes = 1LL << k;
+    tree_level_kernel<T><<<static_cast<unsigned>((nodes + 255) / 256), 256, 0, stream>>>(x, n, k, ord, sq, stats, work);
+    int rc = check_launch(what);
+    if (rc) return rc;
+  }
+  return 0;
+}
+
+int pairwise_sum_f64(const double* x, long long n, double* work, cudaStream_t stream) {
+  return pairwise_sum_tree<double>(x, n, Order3{1, n, 0, 0, 1, true}, 0, nullptr, work, stream, "pairwise_sum_f64");
+}
+
 }  // namespace b2u
 
 using namespace b2u;
@@ -369,18 +397,11 @@ extern "C" int b2u_pre_zscore(float* x, int64_t n, int32_t n0, int32_t n1, int32
   if (n <= 0 || n0 <= 0 || n1 <= 0 || n2 <= 0 || static_cast<long long>(n0) * n1 * n2 != n)
     return set_error(-1, "b2u_pre_zscore: order %dx%dx%d does not cover n=%lld", n0, n1, n2, static_cast<long long>(n));
   Order3 ord{n1, n2, s0, s1, s2, (n0 == 1 && n1 == 1 && s2 == 1)};
-  const int depth = tree_depth(n);
-  if (depth > 40) return set_error(-1, "b2u_pre_zscore: tree depth %d", depth);
   for (int stage = 0; stage < 2; ++stage) {
-    for (int k = depth; k >= 0; --k) {
-      const long long nodes = 1LL << k;
-      tree_level_kernel<<<static_cast<unsigned>((nodes + 255) / 256), 256, 0, stream>>>(x, n, k, ord, stage, stats,
-                                                                                          work);
-      int rc = check_launch("pre_zscore_tree");
-      if (rc) return rc;
-    }
+    int rc = pairwise_sum_tree<float>(x, n, ord, stage, stats, work, stream, "pre_zscore_tree");
+    if (rc) return rc;
     zscore_finalize_kernel<<<1, 1, 0, stream>>>(work, n, stage, stats);
-    int rc = check_launch("pre_zscore_finalize");
+    rc = check_launch("pre_zscore_finalize");
     if (rc) return rc;
   }
   normalize_kernel<<<grid_for(n, 256), 256, 0, stream>>>(x, n, 0, stats, 0.f, 0.f, 0.f, 0.f);

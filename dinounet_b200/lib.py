@@ -102,6 +102,9 @@ SIGNATURES = {
     "b2u_pre_resample3_work_doubles": [i32, i32, i32, i32],
     "b2u_pre_resample3": [vp, i32, i32, i32, i64, i64, i64, i32, i32, i32, vp, vp, vp, vp],
     "b2u_pre_ensemble_f16": [vp, vp, i64, i32, vp],
+    "b2u_eval_masks": [vp, i32, vp, i32, i32, i32, i32, i32, C.POINTER(C.c_int64), i32, i32, i64, vp, vp, vp, vp],
+    "b2u_eval_edt": [vp, i32, i32, i32, C.c_double, C.c_double, C.c_double, vp, vp, vp, vp],
+    "b2u_eval_sum_f64": [vp, i64, vp, vp],
     "b2u_dice_ce_work_doubles": [i32, i32, i64],
     "b2u_dice_ce_forward": [vp, vp, i32, vp, vp, vp, vp, i32, i32, i64, f32, f32, i32, i32, f32, vp],
     "b2u_dice_ce_backward": [vp, vp, i32, vp, vp, i32, i32, i64, f32, f32, i32, i32, f32, f32, vp],

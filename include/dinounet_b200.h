@@ -251,6 +251,31 @@ int b2u_pre_resample3(const float* x, int32_t Z, int32_t h, int32_t w, int64_t s
                       int32_t W, int32_t three_d, const double* consts, double* work, float* out, b2u_stream_t stream);
 int b2u_pre_ensemble_f16(void* acc, const void* x, int64_t n, int32_t divisor, b2u_stream_t stream);
 
+/* ---- Evaluation of predictions against the ground truth (evaluation/evaluate_predictions.py:152-230
+ * `compute_metrics`, HD95 / ASD as medpy's hd95 / asd).  Volumes are C-contiguous [Z, Y, X] (a mask of rank 1 or 2 is
+ * padded with leading axes of size 1, and `ndim` names its true rank).
+ * b2u_eval_masks: one label or region (labels: HOST int64 [n_labels], 1 <= n_labels <= B2U_EVAL_MAX_REGION_LABELS):
+ *   mask = any(seg == labels[j]) with numpy's `==` (exact for the integer dtypes; float32 volumes compare with the
+ *   label rounded to float32); border_* = mask ^ binary_erosion(mask) with face connectivity along the true axes and
+ *   out-of-range neighbours 0 (uint8 0/1 [Z*Y*X]); counts (DEVICE int64 [6], zeroed by the call) = TP, FP, FN, TN over
+ *   the voxels whose reference is not ignore_label (when has_ignore), then the populations of the reference and
+ *   prediction masks over all voxels.  ref_dtype / pred_dtype: B2U_EVAL_* codes; the two may differ.
+ * b2u_eval_edt: dt = scipy distance_transform_edt(border == 0, sampling=(s0, s1, s2)) in float64: the distance of every
+ *   voxel to the nearest border voxel (+inf when the border is empty).  Bit-identical to scipy at integer spacings.
+ *   tmp: double [Z*Y*X]; scratch: int32 [Z*Y*X].  Rows are staged in shared memory, 20 bytes per voxel: X is limited to
+ *   the device's opt-in shared memory per block / 20 (11,622 on an H100).
+ * b2u_eval_sum_f64: work[0] = numpy's pairwise float64 sum of x[n] (np.add.reduce of a contiguous array).  work:
+ *   ceil(n / 8) doubles. */
+enum { B2U_EVAL_U8 = 0, B2U_EVAL_I8 = 1, B2U_EVAL_I16 = 2, B2U_EVAL_U16 = 3, B2U_EVAL_I32 = 4, B2U_EVAL_F32 = 5 };
+#define B2U_EVAL_MAX_REGION_LABELS 8
+int b2u_eval_masks(const void* ref, int32_t ref_dtype, const void* pred, int32_t pred_dtype, int32_t ndim, int32_t Z,
+                   int32_t Y, int32_t X, const int64_t* labels, int32_t n_labels, int32_t has_ignore,
+                   int64_t ignore_label, uint8_t* border_ref, uint8_t* border_pred, int64_t* counts,
+                   b2u_stream_t stream);
+int b2u_eval_edt(const uint8_t* border, int32_t Z, int32_t Y, int32_t X, double s0, double s1, double s2, double* tmp,
+                 int32_t* scratch, double* dt, b2u_stream_t stream);
+int b2u_eval_sum_f64(const double* x, int64_t n, double* work, b2u_stream_t stream);
+
 /* ---- Dice + cross-entropy loss and online-validation statistics on the logits of the forward path
  * (training/loss/compound_losses.py:31-56 `DC_and_CE_loss`, dice.py:72-119 `MemoryEfficientSoftDiceLoss`,
  * robust_ce_loss.py:12-16, built at nnUNetTrainer.py:363-365; consumer nnUNetTrainer.py:961-1005 `validation_step`).
