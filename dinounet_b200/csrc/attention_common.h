@@ -14,8 +14,8 @@ struct alignas(64) AttnMaps {
 struct AttnArgs {
   int BH, heads, ntok, nchunks;
   int q_begin;      // first query row handled by this launch (rows [q_begin, ntok)); keys always span [0, ntok)
-  int qtiles;       // 128-row query tiles per (batch, head)
-  long long items;  // BH * qtiles: one CTA each
+  int qtiles;       // query tiles (attention_tc3_tile_rows rows each) per (batch, head)
+  long long items;  // BH * qtiles, handed out by stride over the persistent CTAs
   float scale_log2e;
   void* out;
 };
@@ -41,6 +41,7 @@ __device__ __forceinline__ float ex2(float x) {
   return r;
 }
 
+int attention_tc3_tile_rows(int head_dim);   // query rows per tile of the kernel for this head dim
 int attention_tc3_dispatch(const AttnMaps& maps, const AttnArgs& a, int head_dim, int dtype, cudaStream_t stream);
 
 }  // namespace b2u

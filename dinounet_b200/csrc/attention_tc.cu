@@ -196,14 +196,15 @@ static int attention_tc_impl(const void* q, const void* k, const void* vt, void*
   a.ntok = ntok;
   a.q_begin = q_begin;
   a.nchunks = (ntok + 127) / 128;
-  a.qtiles = (ntok - q_begin + 127) / 128;
+  const int rows = attention_tc3_tile_rows(head_dim);
+  a.qtiles = (ntok - q_begin + rows - 1) / rows;
   a.items = static_cast<long long>(a.BH) * a.qtiles;
   a.scale_log2e = scale * 1.4426950408889634f;
   a.out = out;
   int rc;
   const uint64_t BH = static_cast<uint64_t>(a.BH), hd = static_cast<uint64_t>(head_dim);
   const uint32_t kc = 128u;
-  if ((rc = make_map_3d(&maps.q, q, dtype, hd, ntok, BH, hd, static_cast<uint64_t>(ntok) * hd, 64, 128))) return rc;
+  if ((rc = make_map_3d(&maps.q, q, dtype, hd, ntok, BH, hd, static_cast<uint64_t>(ntok) * hd, 64, static_cast<uint32_t>(rows)))) return rc;
   if ((rc = make_map_3d(&maps.k, k, dtype, hd, ntok, BH, hd, static_cast<uint64_t>(ntok) * hd, 64, kc))) return rc;
   if ((rc = make_map_3d(&maps.vt, vt, dtype, npad, hd, BH, npad, static_cast<uint64_t>(npad) * hd, 64, static_cast<uint32_t>(head_dim)))) return rc;
   return attention_tc3_dispatch(maps, a, head_dim, dtype, stream);

@@ -11,6 +11,13 @@ __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.a
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Pins the register operands of an in-flight wgmma in program order: the compiler may not move a read or write of r across
+// this point (place it after the wgmma_wait that retires the MMA, and before a wgmma that reads registers written here).
+template <int N>
+__device__ __forceinline__ void wgmma_fence_operand(float (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
+}
 
 // K-major SWIZZLE_128B shared-memory matrix descriptor (sm_90 GMMA layout): [0,14) start >> 4 | [16,30) LBO >> 4 (unused for
 // swizzled K-major, 1) | [32,46) SBO >> 4 (1024 B between 8-row groups) | [62,64) layout 1 = SWIZZLE_128B.  One K step of
@@ -22,6 +29,15 @@ __device__ __forceinline__ uint64_t make_gdesc_k128(uint32_t smem_addr) {
   d |= static_cast<uint64_t>(1024 >> 4) << 32;
   d |= static_cast<uint64_t>(1) << 62;
   return d;
+}
+
+// D[64 x 16] (+)= A[64 x 16, smem] * B[16 x 16, smem]^T
+__device__ __forceinline__ void wgmma_ss_bf16_n16(float (&d)[8], uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(da), "l"(db), "r"(acc));
 }
 
 // D[64 x 32] (+)= A[64 x 16, smem] * B[32 x 16, smem]^T
@@ -65,6 +81,15 @@ __device__ __forceinline__ void wgmma_rs_bf16_n128(float (&d)[64], const uint32_
       "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n}\n"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc));
+}
+
+// D[64 x 16] (+)= A[64 x 16, smem] * B[16 x 16, smem]^T
+__device__ __forceinline__ void wgmma_ss_f16_n16(float (&d)[8], uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(da), "l"(db), "r"(acc));
 }
 
 // D[64 x 32] (+)= A[64 x 16, smem] * B[32 x 16, smem]^T
@@ -140,9 +165,11 @@ __device__ __forceinline__ void wgmma_ss_tf32_n128(float (&d)[64], uint64_t da, 
 // kind: 0 = fp16, 1 = bf16 (the B2U_F16 / B2U_BF16 codes), 2 = tf32
 template <int KIND, int N>
 __device__ __forceinline__ void wgmma_ss(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t acc) {
-  if constexpr (KIND == 0 && N == 32) wgmma_ss_f16_n32(d, da, db, acc);
+  if constexpr (KIND == 0 && N == 16) wgmma_ss_f16_n16(d, da, db, acc);
+  else if constexpr (KIND == 0 && N == 32) wgmma_ss_f16_n32(d, da, db, acc);
   else if constexpr (KIND == 0 && N == 64) wgmma_ss_f16_n64(d, da, db, acc);
   else if constexpr (KIND == 0 && N == 128) wgmma_ss_f16_n128(d, da, db, acc);
+  else if constexpr (KIND == 1 && N == 16) wgmma_ss_bf16_n16(d, da, db, acc);
   else if constexpr (KIND == 1 && N == 32) wgmma_ss_bf16_n32(d, da, db, acc);
   else if constexpr (KIND == 1 && N == 64) wgmma_ss_bf16_n64(d, da, db, acc);
   else if constexpr (KIND == 1 && N == 128) wgmma_ss_bf16_n128(d, da, db, acc);

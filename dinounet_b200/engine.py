@@ -345,8 +345,9 @@ class ForwardEngine:
             plan.keep.append(qp)
             plan.rope_sites.append((len(plan.calls), i, _patch_qkv_rope))
             plan.add(f"b{i}.qkv", lib.b2u_qkv_rope, C.byref(qp))
-            # one launch over all ntok query rows (the 5 cls/storage rows form a ninth query tile whose out-of-range row
-            # quarters only run the barrier protocol; b2u_attention_rows remains available for a split launch)
+            # one launch over all ntok query rows (the 5 cls/storage rows fall in the last query tile, whose consumer
+            # warpgroups with no valid rows only keep the barrier protocol; b2u_attention_rows remains available for a
+            # split launch)
             if hd == 64:
                 plan.add(f"b{i}.attn", lib.b2u_attention_tc, _ptr(Q), _ptr(K_), _ptr(V), _ptr(O), B, Hh, N, npad, 0,
                          hd ** -0.5, vt)
