@@ -10,23 +10,32 @@
 // Region-based training (DC_and_BCE_loss, compound_losses.py:59-99, sigmoid Dice with do_bg, optional ignore channel)
 // uses the same three-step shape on [B, R, plane] logits and [B, R(+1), plane] real-valued targets.
 //
-// Data-parallel batch Dice (dice.py:106-110): the split entry points stop after the statistics pass with the per-class
+// Data-parallel batch Dice (dice.py:106-110): given a batch_sums buffer, the statistics pass also writes the per-class
 // batch sums [C][3] (intersect, sum_pred, sum_gt; fp64, on the device), which the caller all-reduces across ranks before
-// the finalisation.  The backward takes the incoming gradient as device scalars: the CE/BCE part is scaled by the local
-// one, the Dice part by the all-reduced one (the backward of AllGatherGrad, ddp_allgather.py:43-48).  No host sync.
+// the finalisation; without one (label maps only), the finalisation and the gradient sum the per-sample records
+// themselves, in the same order.  The backward may take the incoming gradient as device scalars: the CE/BCE part is
+// scaled by the local one, the Dice part by the all-reduced one (the backward of AllGatherGrad, ddp_allgather.py:43-48).
+// No host sync.
 //
-// An ignore label (DC_and_CE_loss(..., ignore_label), compound_losses.py:38-53) takes the split entry points with the
-// kernels' IGN instantiations: masked sums, a valid-pixel count per sample, CE over the valid pixels only.
+// An ignore label (DC_and_CE_loss(..., ignore_label), compound_losses.py:38-53) runs the kernels' IGN instantiations:
+// masked sums, a valid-pixel count per sample, CE over the valid pixels only.
 #include "common.cuh"
 #include "host_util.h"
 #include "gemm_common.h"
 #include "../../include/dinounet_b200.h"
 
 #include <algorithm>
+#include <initializer_list>
+#include <type_traits>
+#include <utility>
 
 namespace b2u {
 
 constexpr int kStat = 6;  // per (sample, class): intersect, sum_pred, sum_gt, tp, fp, fn
+
+// one sample's record of label-map sums: kStat per class, then the CE sum (and, with an ignore label, the valid-pixel
+// count)
+__host__ __device__ constexpr int record_len(int C, bool ign) { return C * kStat + 1 + (ign ? 1 : 0); }
 
 template <typename L> __device__ __forceinline__ int load_label(const void* t, long long i) {
   return static_cast<int>(static_cast<const L*>(t)[i]);
@@ -101,7 +110,7 @@ __global__ void __launch_bounds__(256) loss_stats_kernel(const float* __restrict
                                                          long long plane, int ignore_label) {
   const int b = blockIdx.y;
   const float* zb = logits + static_cast<long long>(b) * C * plane;
-  constexpr int K = C * kStat + 1 + IGN;  // then the CE sum (and the valid-pixel count)
+  constexpr int K = record_len(C, IGN);
   float acc[K];
 #pragma unroll
   for (int k = 0; k < K; ++k) acc[k] = 0.f;
@@ -142,20 +151,34 @@ __device__ __forceinline__ void reduce_sample_stats(const double* __restrict__ p
   }
 }
 
-// bsum[c][3] = (intersect, sum_pred, sum_gt) of class c over the batch: per sample in block order, then in sample
-// order, which is the order the fused finalisation sums in.  K = per-sample record length; class c's record at c*kStat.
+// (intersect, sum_pred, sum_gt) of class c: gsum[c] when the batch sums [C][3] are given, else the records of samples
+// b0 <= b < b1 summed in sample order from 0 -- the order dice_batch_sums_kernel sums in, so that skipping it changes no
+// bit.  K = per-sample record length; class c's record at c*kStat.
+__device__ __forceinline__ void dice_sums(const double* __restrict__ gsum, const double* __restrict__ stats, int K, int c,
+                                          int b0, int b1, double& I, double& P, double& G) {
+  if (gsum) {
+    I = gsum[c * 3];
+    P = gsum[c * 3 + 1];
+    G = gsum[c * 3 + 2];
+    return;
+  }
+  I = P = G = 0;
+  for (int b = b0; b < b1; ++b) {
+    I += stats[b * K + c * kStat];
+    P += stats[b * K + c * kStat + 1];
+    G += stats[b * K + c * kStat + 2];
+  }
+}
+
+// bsum[c][3] = (intersect, sum_pred, sum_gt) of class c over the batch: per sample in block order, then in sample order.
 // The per-sample sums go through `stats` (B*K doubles) so that every thread of the block takes part in the long first
 // level, instead of one thread per output running over all B*nblk partials.
 __global__ void dice_batch_sums_kernel(const double* __restrict__ partial, double* __restrict__ stats,
                                        double* __restrict__ bsum, int B, int C, int K, int nblk) {
   reduce_sample_stats(partial, stats, B, K, nblk);
   __syncthreads();
-  for (int j = threadIdx.x; j < C * 3; j += blockDim.x) {
-    const int c = j / 3, s = j - c * 3;
-    double v = 0;
-    for (int b = 0; b < B; ++b) v += stats[b * K + c * kStat + s];
-    bsum[j] = v;
-  }
+  for (int c = threadIdx.x; c < C; c += blockDim.x)
+    dice_sums(nullptr, stats, K, c, 0, B, bsum[c * 3], bsum[c * 3 + 1], bsum[c * 3 + 2]);
 }
 
 // stats: double [B][C*6 + 1 (+1 with IGN)] (the sample's CE sum, and its valid-pixel count).  out: float[3] = loss, ce,
@@ -165,7 +188,7 @@ __global__ void loss_finalize_kernel(const double* __restrict__ partial, double*
                                      const double* __restrict__ gsum, float* __restrict__ out,
                                      int64_t* __restrict__ tpfpfn, int B, int C, int nblk, long long plane, float w_ce,
                                      float w_dice, int batch_dice, int do_bg, float smooth) {
-  const int K = C * kStat + 1 + IGN;
+  const int K = record_len(C, IGN);
   reduce_sample_stats(partial, stats, B, K, nblk);
   __syncthreads();
   if (threadIdx.x != 0) return;
@@ -178,33 +201,15 @@ __global__ void loss_finalize_kernel(const double* __restrict__ partial, double*
   } else {
     ce /= static_cast<double>(B) * static_cast<double>(plane);
   }
-  const int c0 = do_bg ? 0 : 1;
+  const int c0 = do_bg ? 0 : 1, nd = batch_dice ? 1 : B;  // Dice terms: one of the batch, or one per sample
   double dc = 0;
-  if (batch_dice) {
+  for (int d = 0; d < nd; ++d)
     for (int c = c0; c < C; ++c) {
-      double I = 0, P = 0, G = 0;
-      if (gsum) {
-        I = gsum[c * 3];
-        P = gsum[c * 3 + 1];
-        G = gsum[c * 3 + 2];
-      } else {
-        for (int b = 0; b < B; ++b) {
-          I += stats[b * K + c * kStat];
-          P += stats[b * K + c * kStat + 1];
-          G += stats[b * K + c * kStat + 2];
-        }
-      }
+      double I, P, G;
+      dice_sums(batch_dice ? gsum : nullptr, stats, K, c, batch_dice ? 0 : d, batch_dice ? B : d + 1, I, P, G);
       dc += (2 * I + smooth) / fmax(G + P + smooth, 1e-8);
     }
-    dc /= (C - c0);
-  } else {
-    for (int b = 0; b < B; ++b)
-      for (int c = c0; c < C; ++c) {
-        const double I = stats[b * K + c * kStat], P = stats[b * K + c * kStat + 1], G = stats[b * K + c * kStat + 2];
-        dc += (2 * I + smooth) / fmax(G + P + smooth, 1e-8);
-      }
-    dc /= static_cast<double>(B) * (C - c0);
-  }
+  dc /= static_cast<double>(nd) * (C - c0);
   out[1] = static_cast<float>(ce);
   out[2] = static_cast<float>(-dc);
   out[0] = static_cast<float>(w_ce * ce - w_dice * dc);
@@ -227,7 +232,7 @@ __global__ void __launch_bounds__(256) loss_grad_kernel(const float* __restrict_
                                                         const float* __restrict__ ce_scale,
                                                         const float* __restrict__ dice_scale, int ignore_label) {
   const int b = blockIdx.y;
-  constexpr int K = C * kStat + 1 + IGN;
+  constexpr int K = record_len(C, IGN);
   // per-class dice coefficients a_c, b_c with d(dice term)/dp_c = a_c * y_c + b_c
   __shared__ float sa[C], sb[C], s_ce;
   if (IGN && threadIdx.x == 32) {
@@ -293,7 +298,7 @@ __global__ void __launch_bounds__(256) loss_grad_kernel(const float* __restrict_
 
 // ---- region-based (sigmoid) Dice + BCE.  Per (sample, region): intersect, sum_pred, sum_gt over valid pixels and the
 // validation tp, fp, fn of sigmoid(z) > 0.5 weighted by 1 - t_ign; per sample: BCE sum over valid pixels, valid count.
-constexpr int kRegionExtra = 2;
+__host__ __device__ constexpr int region_record_len(int R) { return R * kStat + 2; }
 
 __device__ __forceinline__ float bce_with_logits(float z, float y) {
   return fmaxf(z, 0.f) - z * y + log1pf(expf(-fabsf(z)));
@@ -306,7 +311,7 @@ __global__ void __launch_bounds__(256) region_stats_kernel(const float* __restri
   const int b = blockIdx.y;
   const float* zb = logits + static_cast<long long>(b) * R * plane;
   const long long tb = static_cast<long long>(b) * (R + has_ignore) * plane;
-  constexpr int K = R * kStat + kRegionExtra;
+  constexpr int K = region_record_len(R);
   float acc[K];
 #pragma unroll
   for (int k = 0; k < K; ++k) acc[k] = 0.f;
@@ -342,7 +347,7 @@ __global__ void region_finalize_kernel(const double* __restrict__ partial, doubl
                                        const double* __restrict__ bsum, float* __restrict__ out,
                                        float* __restrict__ tpfpfn, int B, int R, int nblk, long long plane, float w_ce,
                                        float w_dice, int batch_dice, int has_ignore, float smooth) {
-  const int K = R * kStat + kRegionExtra;
+  const int K = region_record_len(R);
   reduce_sample_stats(partial, stats, B, K, nblk);
   __syncthreads();
   if (threadIdx.x != 0) return;
@@ -387,7 +392,7 @@ __global__ void __launch_bounds__(256) region_grad_kernel(const float* __restric
                                                           const float* __restrict__ ce_scale,
                                                           const float* __restrict__ dice_scale) {
   const int b = blockIdx.y;
-  constexpr int K = R * kStat + kRegionExtra;
+  constexpr int K = region_record_len(R);
   // d(dice term)/dx_r = (a_r * y_r + b_r) * m;  d BCE / dz_r = bce_w * (x_r - y_r) * m
   __shared__ float sa[R], sb[R], s_bce;
   if (threadIdx.x < R) {
@@ -443,221 +448,121 @@ static int grad_blocks(long long plane) {
   return static_cast<int>(std::max<long long>(1, std::min<long long>((plane + 1023) / 1024, 4096)));
 }
 
-extern "C" int64_t b2u_dice_ce_work_doubles(int32_t B, int32_t C, int64_t plane) {
-  return static_cast<int64_t>(B) * stats_blocks(plane) * (C * kStat + 1) + static_cast<int64_t>(B) * (C * kStat + 1);
-}
-
-extern "C" int64_t b2u_dice_ce_ign_work_doubles(int32_t B, int32_t C, int64_t plane) {
-  return static_cast<int64_t>(B) * stats_blocks(plane) * (C * kStat + 2) + static_cast<int64_t>(B) * (C * kStat + 2);
-}
-
-extern "C" int64_t b2u_dice_bce_work_doubles(int32_t B, int32_t R, int64_t plane) {
-  const int64_t K = R * kStat + kRegionExtra;
+// work: B*nblk block partials of K doubles each, then the B per-sample records (K = the record length)
+static int64_t work_doubles(int32_t B, int64_t plane, int K) {
   return static_cast<int64_t>(B) * stats_blocks(plane) * K + static_cast<int64_t>(B) * K;
 }
 
-// one instantiation per class count: every per-class sum lives in a named register (large counts spill, which is fine
-// for a pass that is run once per step)
-#define B2U_LOSS_SWITCH(C, BODY)                                                               \
-  switch (C) {                                                                                 \
-    case 2: { constexpr int CC = 2; BODY } break;                                        \
-    case 3: { constexpr int CC = 3; BODY } break;                                        \
-    case 4: { constexpr int CC = 4; BODY } break;                                        \
-    case 5: { constexpr int CC = 5; BODY } break;                                        \
-    case 6: { constexpr int CC = 6; BODY } break;                                        \
-    case 7: { constexpr int CC = 7; BODY } break;                                        \
-    case 8: { constexpr int CC = 8; BODY } break;                                        \
-    case 9: { constexpr int CC = 9; BODY } break;                                        \
-    case 10: { constexpr int CC = 10; BODY } break;                                        \
-    case 11: { constexpr int CC = 11; BODY } break;                                        \
-    case 12: { constexpr int CC = 12; BODY } break;                                        \
-    case 13: { constexpr int CC = 13; BODY } break;                                        \
-    case 14: { constexpr int CC = 14; BODY } break;                                        \
-    case 15: { constexpr int CC = 15; BODY } break;                                        \
-    case 16: { constexpr int CC = 16; BODY } break;                                        \
-    case 17: { constexpr int CC = 17; BODY } break;                                        \
-    case 18: { constexpr int CC = 18; BODY } break;                                        \
-    case 19: { constexpr int CC = 19; BODY } break;                                        \
-    case 20: { constexpr int CC = 20; BODY } break;                                        \
-    case 21: { constexpr int CC = 21; BODY } break;                                        \
-    case 22: { constexpr int CC = 22; BODY } break;                                        \
-    case 23: { constexpr int CC = 23; BODY } break;                                        \
-    case 24: { constexpr int CC = 24; BODY } break;                                        \
-    case 25: { constexpr int CC = 25; BODY } break;                                        \
-    case 26: { constexpr int CC = 26; BODY } break;                                        \
-    case 27: { constexpr int CC = 27; BODY } break;                                        \
-    case 28: { constexpr int CC = 28; BODY } break;                                        \
-    case 29: { constexpr int CC = 29; BODY } break;                                        \
-    case 30: { constexpr int CC = 30; BODY } break;                                        \
-    case 31: { constexpr int CC = 31; BODY } break;                                        \
-    case 32: { constexpr int CC = 32; BODY } break;                                        \
-    default: return set_error(-1, "dice_ce: %d classes not in [2, 32]", C);                    \
-  }
-
-// regions: one instantiation per region count, 1 <= R <= 32 (a single region is one sigmoid head)
-#define B2U_REGION_SWITCH(R, BODY)    \
-  if ((R) == 1) {                     \
-    constexpr int CC = 1;             \
-    BODY                              \
-  } else {                            \
-    B2U_LOSS_SWITCH(R, BODY)          \
-  }
-
-template <bool IGN = false>
-static int dice_ce_stats(const float* logits, const void* target, int32_t target_kind, double* work,
-                         int32_t* bad_label, int32_t B, int32_t C, int64_t plane, cudaStream_t stream,
-                         int32_t ignore_label = 0) {
-  const int nblk = stats_blocks(plane);
-  dim3 grid(nblk, B);
-  B2U_LOSS_SWITCH(C, (loss_stats_kernel<CC, IGN><<<grid, 256, 0, stream>>>(logits, target, target_kind, work,
-                                                                           bad_label, plane, ignore_label));)
-  return check_launch("dice_ce_stats");
+template <typename T> static T* sample_records(T* work, int32_t B, int64_t plane, int K) {
+  return work + static_cast<int64_t>(B) * stats_blocks(plane) * K;
 }
 
-extern "C" int b2u_dice_ce_forward(const float* logits, const void* target, int32_t target_kind, double* work,
-                                   float* out3, int64_t* tp_fp_fn, int32_t* bad_label, int32_t B, int32_t C,
-                                   int64_t plane, float weight_ce, float weight_dice, int32_t batch_dice, int32_t do_bg,
-                                   float smooth, b2u_stream_t stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (!logits || !target || !work || !out3 || !bad_label) return set_error(-1, "b2u_dice_ce_forward: null pointer");
-  if (B <= 0 || plane <= 0 || target_kind < 0 || target_kind > 3) return set_error(-1, "b2u_dice_ce_forward: bad argument");
-  if (!do_bg && C < 2) return set_error(-1, "b2u_dice_ce_forward: do_bg=0 needs >= 2 classes");
-  if (int rc = dice_ce_stats(logits, target, target_kind, work, bad_label, B, C, plane, stream)) return rc;
-  const int nblk = stats_blocks(plane);
-  double* stats = work + static_cast<int64_t>(B) * nblk * (C * kStat + 1);
-  loss_finalize_kernel<<<1, 256, 0, stream>>>(work, stats, nullptr, out3, tp_fp_fn, B, C, nblk, plane, weight_ce,
-                                              weight_dice, batch_dice, do_bg, smooth);
-  return check_launch("dice_ce_finalize");
+// f(std::integral_constant<int, n>{}) for the count n in [Lo, Hi] (the caller checked the range): one instantiation per
+// count, so that every per-class sum lives in a named register (large counts spill, which is fine for a pass that is
+// run once per step)
+template <int Lo, typename F, int... I> static void with_count(int n, F&& f, std::integer_sequence<int, I...>) {
+  (void)((n == Lo + I && (f(std::integral_constant<int, Lo + I>{}), true)) || ...);
+}
+template <int Lo, int Hi, typename F> static void with_count(int n, F&& f) {
+  with_count<Lo>(n, f, std::make_integer_sequence<int, Hi - Lo + 1>{});
 }
 
-extern "C" int b2u_dice_ce_stats(const float* logits, const void* target, int32_t target_kind, double* work,
-                                 double* batch_sums, int32_t* bad_label, int32_t B, int32_t C, int64_t plane,
-                                 b2u_stream_t stream_) {
+// label maps: f(classes, ignore label?) as compile-time constants, 2 <= C <= 32
+template <typename F> static void with_classes(int C, int has_ignore, F&& f) {
+  if (has_ignore)
+    with_count<2, 32>(C, [&](auto c) { f(c, std::true_type{}); });
+  else
+    with_count<2, 32>(C, [&](auto c) { f(c, std::false_type{}); });
+}
+
+// argument checks of the label-map entry points: the buffers the call needs, then the sizes (the finalisation reads
+// no target and passes target_kind 0)
+static int dice_ce_args(const char* fn, std::initializer_list<const void*> bufs, int32_t target_kind, int32_t B,
+                        int32_t C, int64_t plane) {
+  for (const void* p : bufs)
+    if (!p) return set_error(-1, "%s: null pointer", fn);
+  if (B <= 0 || plane <= 0 || target_kind < 0 || target_kind > 3) return set_error(-1, "%s: bad argument", fn);
+  if (C < 2 || C > 32) return set_error(-1, "dice_ce: %d classes not in [2, 32]", C);
+  return 0;
+}
+
+extern "C" int64_t b2u_dice_ce_work_doubles(int32_t B, int32_t C, int64_t plane, int32_t has_ignore) {
+  return work_doubles(B, plane, record_len(C, has_ignore));
+}
+
+extern "C" int b2u_dice_ce_stats(const float* logits, const void* target, int32_t target_kind, int32_t has_ignore,
+                                 int32_t ignore_label, double* work, double* batch_sums, int32_t* bad_label, int32_t B,
+                                 int32_t C, int64_t plane, b2u_stream_t stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (!logits || !target || !work || !batch_sums || !bad_label) return set_error(-1, "b2u_dice_ce_stats: null pointer");
-  if (B <= 0 || plane <= 0 || target_kind < 0 || target_kind > 3) return set_error(-1, "b2u_dice_ce_stats: bad argument");
-  if (int rc = dice_ce_stats(logits, target, target_kind, work, bad_label, B, C, plane, stream)) return rc;
-  const int nblk = stats_blocks(plane), K = C * kStat + 1;
-  dice_batch_sums_kernel<<<1, 256, 0, stream>>>(work, work + static_cast<int64_t>(B) * nblk * K, batch_sums, B, C, K,
-                                                nblk);
+  if (int rc = dice_ce_args("b2u_dice_ce_stats", {logits, target, work, bad_label}, target_kind, B, C, plane)) return rc;
+  const int nblk = stats_blocks(plane), K = record_len(C, has_ignore);
+  with_classes(C, has_ignore, [&](auto c, auto ign) {
+    loss_stats_kernel<decltype(c)::value, decltype(ign)::value><<<dim3(nblk, B), 256, 0, stream>>>(
+        logits, target, target_kind, work, bad_label, plane, ignore_label);
+  });
+  if (int rc = check_launch("dice_ce_stats")) return rc;
+  if (!batch_sums) return 0;
+  dice_batch_sums_kernel<<<1, 256, 0, stream>>>(work, sample_records(work, B, plane, K), batch_sums, B, C, K, nblk);
   return check_launch("dice_ce_batch_sums");
 }
 
 extern "C" int b2u_dice_ce_finalize(double* work, const double* batch_sums, float* out3, int64_t* tp_fp_fn, int32_t B,
-                                    int32_t C, int64_t plane, float weight_ce, float weight_dice, int32_t batch_dice,
-                                    int32_t do_bg, float smooth, b2u_stream_t stream_) {
+                                    int32_t C, int64_t plane, int32_t has_ignore, float weight_ce, float weight_dice,
+                                    int32_t batch_dice, int32_t do_bg, float smooth, b2u_stream_t stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (!work || !batch_sums || !out3) return set_error(-1, "b2u_dice_ce_finalize: null pointer");
-  if (B <= 0 || plane <= 0 || C < 2 || C > 32) return set_error(-1, "b2u_dice_ce_finalize: bad argument");
-  const int nblk = stats_blocks(plane);
-  double* stats = work + static_cast<int64_t>(B) * nblk * (C * kStat + 1);
-  loss_finalize_kernel<<<1, 256, 0, stream>>>(work, stats, batch_sums, out3, tp_fp_fn, B, C, nblk, plane, weight_ce,
-                                              weight_dice, batch_dice, do_bg, smooth);
+  if (int rc = dice_ce_args("b2u_dice_ce_finalize", {work, out3}, 0, B, C, plane)) return rc;
+  double* stats = sample_records(work, B, plane, record_len(C, has_ignore));
+  auto* finalize = has_ignore ? loss_finalize_kernel<true> : loss_finalize_kernel<false>;
+  finalize<<<1, 256, 0, stream>>>(work, stats, batch_sums, out3, tp_fp_fn, B, C, stats_blocks(plane), plane, weight_ce,
+                                  weight_dice, batch_dice, do_bg, smooth);
   return check_launch("dice_ce_finalize");
 }
 
-template <bool IGN = false>
-static int dice_ce_grad(const float* logits, const void* target, int32_t target_kind, const double* work,
-                        const double* batch_sums, float* grad_logits, int32_t B, int32_t C, int64_t plane,
-                        float weight_ce, float weight_dice, int32_t batch_dice, int32_t do_bg, float smooth,
-                        float grad_scale, const float* ce_scale, const float* dice_scale, cudaStream_t stream,
-                        int32_t ignore_label = 0) {
-  if (!logits || !target || !work || !grad_logits) return set_error(-1, "b2u_dice_ce_backward: null pointer");
-  if (target_kind < 0 || target_kind > 3) return set_error(-1, "b2u_dice_ce_backward: bad target kind");
-  const int nblk = stats_blocks(plane);
-  const double* stats = work + static_cast<int64_t>(B) * nblk * (C * kStat + 1 + IGN);
-  dim3 grid(grad_blocks(plane), B);
-  B2U_LOSS_SWITCH(C, (loss_grad_kernel<CC, IGN><<<grid, 256, 0, stream>>>(logits, target, target_kind, stats,
-                                                                          batch_sums, grad_logits, B, plane, weight_ce,
-                                                                          weight_dice, batch_dice, do_bg, smooth,
-                                                                          grad_scale, ce_scale, dice_scale,
-                                                                          ignore_label));)
+extern "C" int b2u_dice_ce_backward(const float* logits, const void* target, int32_t target_kind, int32_t has_ignore,
+                                    int32_t ignore_label, const double* work, const double* batch_sums,
+                                    float* grad_logits, int32_t B, int32_t C, int64_t plane, float weight_ce,
+                                    float weight_dice, int32_t batch_dice, int32_t do_bg, float smooth,
+                                    const float* ce_scale, const float* dice_scale, b2u_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (int rc = dice_ce_args("b2u_dice_ce_backward", {logits, target, work, grad_logits}, target_kind, B, C, plane))
+    return rc;
+  const double* stats = sample_records(work, B, plane, record_len(C, has_ignore));
+  with_classes(C, has_ignore, [&](auto c, auto ign) {
+    loss_grad_kernel<decltype(c)::value, decltype(ign)::value><<<dim3(grad_blocks(plane), B), 256, 0, stream>>>(
+        logits, target, target_kind, stats, batch_sums, grad_logits, B, plane, weight_ce, weight_dice, batch_dice,
+        do_bg, smooth, 1.f, ce_scale, dice_scale, ignore_label);
+  });
   return check_launch("dice_ce_backward");
 }
 
-extern "C" int b2u_dice_ce_backward(const float* logits, const void* target, int32_t target_kind, const double* work,
-                                    float* grad_logits, int32_t B, int32_t C, int64_t plane, float weight_ce,
-                                    float weight_dice, int32_t batch_dice, int32_t do_bg, float smooth,
-                                    float grad_scale, b2u_stream_t stream_) {
-  return dice_ce_grad(logits, target, target_kind, work, nullptr, grad_logits, B, C, plane, weight_ce, weight_dice,
-                      batch_dice, do_bg, smooth, grad_scale, nullptr, nullptr, static_cast<cudaStream_t>(stream_));
-}
-
-extern "C" int b2u_dice_ce_backward_scaled(const float* logits, const void* target, int32_t target_kind,
-                                           const double* work, const double* batch_sums, float* grad_logits, int32_t B,
-                                           int32_t C, int64_t plane, float weight_ce, float weight_dice,
-                                           int32_t batch_dice, int32_t do_bg, float smooth, const float* ce_scale,
-                                           const float* dice_scale, b2u_stream_t stream_) {
-  if (!batch_sums || !ce_scale || !dice_scale) return set_error(-1, "b2u_dice_ce_backward_scaled: null pointer");
-  return dice_ce_grad(logits, target, target_kind, work, batch_sums, grad_logits, B, C, plane, weight_ce, weight_dice,
-                      batch_dice, do_bg, smooth, 1.f, ce_scale, dice_scale, static_cast<cudaStream_t>(stream_));
-}
-
-// ---- the same loss with an ignore label (label maps of sparsely annotated datasets): split forward as above, the
-// per-sample records carry the valid-pixel count, the backward takes its scales from the device.
-extern "C" int b2u_dice_ce_ign_stats(const float* logits, const void* target, int32_t target_kind, int32_t ignore_label,
-                                     double* work, double* batch_sums, int32_t* bad_label, int32_t B, int32_t C,
-                                     int64_t plane, b2u_stream_t stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (!logits || !target || !work || !batch_sums || !bad_label)
-    return set_error(-1, "b2u_dice_ce_ign_stats: null pointer");
-  if (B <= 0 || plane <= 0 || target_kind < 0 || target_kind > 3)
-    return set_error(-1, "b2u_dice_ce_ign_stats: bad argument");
-  if (int rc = dice_ce_stats<true>(logits, target, target_kind, work, bad_label, B, C, plane, stream, ignore_label))
-    return rc;
-  const int nblk = stats_blocks(plane), K = C * kStat + 2;
-  dice_batch_sums_kernel<<<1, 256, 0, stream>>>(work, work + static_cast<int64_t>(B) * nblk * K, batch_sums, B, C, K,
-                                                nblk);
-  return check_launch("dice_ce_ign_batch_sums");
-}
-
-extern "C" int b2u_dice_ce_ign_finalize(double* work, const double* batch_sums, float* out3, int64_t* tp_fp_fn,
-                                        int32_t B, int32_t C, int64_t plane, float weight_ce, float weight_dice,
-                                        int32_t batch_dice, int32_t do_bg, float smooth, b2u_stream_t stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (!work || !batch_sums || !out3) return set_error(-1, "b2u_dice_ce_ign_finalize: null pointer");
-  if (B <= 0 || plane <= 0 || C < 2 || C > 32) return set_error(-1, "b2u_dice_ce_ign_finalize: bad argument");
-  const int nblk = stats_blocks(plane);
-  double* stats = work + static_cast<int64_t>(B) * nblk * (C * kStat + 2);
-  loss_finalize_kernel<true><<<1, 256, 0, stream>>>(work, stats, batch_sums, out3, tp_fp_fn, B, C, nblk, plane,
-                                                    weight_ce, weight_dice, batch_dice, do_bg, smooth);
-  return check_launch("dice_ce_ign_finalize");
-}
-
-extern "C" int b2u_dice_ce_ign_backward(const float* logits, const void* target, int32_t target_kind,
-                                        int32_t ignore_label, const double* work, const double* batch_sums,
-                                        float* grad_logits, int32_t B, int32_t C, int64_t plane, float weight_ce,
-                                        float weight_dice, int32_t batch_dice, int32_t do_bg, float smooth,
-                                        const float* ce_scale, const float* dice_scale, b2u_stream_t stream_) {
-  if (!batch_sums || !ce_scale || !dice_scale) return set_error(-1, "b2u_dice_ce_ign_backward: null pointer");
-  if (B <= 0 || plane <= 0) return set_error(-1, "b2u_dice_ce_ign_backward: bad argument");
-  return dice_ce_grad<true>(logits, target, target_kind, work, batch_sums, grad_logits, B, C, plane, weight_ce,
-                            weight_dice, batch_dice, do_bg, smooth, 1.f, ce_scale, dice_scale,
-                            static_cast<cudaStream_t>(stream_), ignore_label);
-}
-
-static int region_args(const char* fn, const float* logits, const void* target, int32_t target_kind, int32_t B,
-                       int32_t R, int64_t plane) {
-  if (!logits || !target) return set_error(-1, "%s: null pointer", fn);
+// ---- regions (1 <= R <= 32: a single region is one sigmoid head).  The region kernels take the batch Dice from
+// batch_sums only, so that buffer is required.
+static int dice_bce_args(const char* fn, std::initializer_list<const void*> bufs, int32_t target_kind, int32_t B,
+                         int32_t R, int64_t plane) {
+  for (const void* p : bufs)
+    if (!p) return set_error(-1, "%s: null pointer", fn);
   if (B <= 0 || plane <= 0 || target_kind < 0 || target_kind > 3) return set_error(-1, "%s: bad argument", fn);
   if (R < 1 || R > 32) return set_error(-1, "%s: %d regions not in [1, 32]", fn, R);
   return 0;
+}
+
+extern "C" int64_t b2u_dice_bce_work_doubles(int32_t B, int32_t R, int64_t plane) {
+  return work_doubles(B, plane, region_record_len(R));
 }
 
 extern "C" int b2u_dice_bce_stats(const float* logits, const void* target, int32_t target_kind, int32_t has_ignore,
                                   double* work, double* batch_sums, int32_t B, int32_t R, int64_t plane,
                                   b2u_stream_t stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (int rc = region_args("b2u_dice_bce_stats", logits, target, target_kind, B, R, plane)) return rc;
-  if (!work || !batch_sums) return set_error(-1, "b2u_dice_bce_stats: null pointer");
-  const int nblk = stats_blocks(plane), ign = has_ignore ? 1 : 0;
-  dim3 grid(nblk, B);
-  B2U_REGION_SWITCH(R, (region_stats_kernel<CC><<<grid, 256, 0, stream>>>(logits, target, target_kind, ign, work,
-                                                                          plane));)
+  if (int rc = dice_bce_args("b2u_dice_bce_stats", {logits, target, work, batch_sums}, target_kind, B, R, plane))
+    return rc;
+  const int nblk = stats_blocks(plane), K = region_record_len(R), ign = has_ignore ? 1 : 0;
+  with_count<1, 32>(R, [&](auto r) {
+    region_stats_kernel<decltype(r)::value><<<dim3(nblk, B), 256, 0, stream>>>(logits, target, target_kind, ign, work,
+                                                                                plane);
+  });
   if (int rc = check_launch("dice_bce_stats")) return rc;
-  const int K = R * kStat + kRegionExtra;
-  dice_batch_sums_kernel<<<1, 256, 0, stream>>>(work, work + static_cast<int64_t>(B) * nblk * K, batch_sums, B, R, K,
-                                                nblk);
+  dice_batch_sums_kernel<<<1, 256, 0, stream>>>(work, sample_records(work, B, plane, K), batch_sums, B, R, K, nblk);
   return check_launch("dice_bce_batch_sums");
 }
 
@@ -665,12 +570,10 @@ extern "C" int b2u_dice_bce_finalize(double* work, const double* batch_sums, flo
                                      int32_t R, int64_t plane, float weight_ce, float weight_dice, int32_t batch_dice,
                                      int32_t has_ignore, float smooth, b2u_stream_t stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (!work || !batch_sums || !out3) return set_error(-1, "b2u_dice_bce_finalize: null pointer");
-  if (B <= 0 || plane <= 0 || R < 1 || R > 32) return set_error(-1, "b2u_dice_bce_finalize: bad argument");
-  const int nblk = stats_blocks(plane);
-  double* stats = work + static_cast<int64_t>(B) * nblk * (R * kStat + kRegionExtra);
-  region_finalize_kernel<<<1, 256, 0, stream>>>(work, stats, batch_sums, out3, tp_fp_fn, B, R, nblk, plane, weight_ce,
-                                                weight_dice, batch_dice, has_ignore ? 1 : 0, smooth);
+  if (int rc = dice_bce_args("b2u_dice_bce_finalize", {work, batch_sums, out3}, 0, B, R, plane)) return rc;
+  double* stats = sample_records(work, B, plane, region_record_len(R));
+  region_finalize_kernel<<<1, 256, 0, stream>>>(work, stats, batch_sums, out3, tp_fp_fn, B, R, stats_blocks(plane),
+                                                plane, weight_ce, weight_dice, batch_dice, has_ignore ? 1 : 0, smooth);
   return check_launch("dice_bce_finalize");
 }
 
@@ -680,16 +583,17 @@ extern "C" int b2u_dice_bce_backward(const float* logits, const void* target, in
                                      float smooth, const float* ce_scale, const float* dice_scale,
                                      b2u_stream_t stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (int rc = region_args("b2u_dice_bce_backward", logits, target, target_kind, B, R, plane)) return rc;
-  if (!work || !batch_sums || !grad_logits || !ce_scale || !dice_scale)
-    return set_error(-1, "b2u_dice_bce_backward: null pointer");
-  const int nblk = stats_blocks(plane), ign = has_ignore ? 1 : 0;
-  const double* stats = work + static_cast<int64_t>(B) * nblk * (R * kStat + kRegionExtra);
-  dim3 grid(grad_blocks(plane), B);
-  B2U_REGION_SWITCH(R, (region_grad_kernel<CC><<<grid, 256, 0, stream>>>(logits, target, target_kind, ign, stats,
-                                                                         batch_sums, grad_logits, B, plane, weight_ce,
-                                                                         weight_dice, batch_dice, smooth, ce_scale,
-                                                                         dice_scale));)
+  if (int rc = dice_bce_args("b2u_dice_bce_backward",
+                             {logits, target, work, batch_sums, grad_logits, ce_scale, dice_scale}, target_kind, B, R,
+                             plane))
+    return rc;
+  const double* stats = sample_records(work, B, plane, region_record_len(R));
+  const int ign = has_ignore ? 1 : 0;
+  with_count<1, 32>(R, [&](auto r) {
+    region_grad_kernel<decltype(r)::value><<<dim3(grad_blocks(plane), B), 256, 0, stream>>>(
+        logits, target, target_kind, ign, stats, batch_sums, grad_logits, B, plane, weight_ce, weight_dice, batch_dice,
+        smooth, ce_scale, dice_scale);
+  });
   return check_launch("dice_bce_backward");
 }
 

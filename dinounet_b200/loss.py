@@ -17,8 +17,8 @@ gradients (the AllGatherGrad backward, ddp_allgather.py:43-48).  Both happen on 
 
 Ignore label of the softmax loss (`DC_and_CE_loss(..., ignore_label=N)`, sparsely annotated label maps): pixels labelled N
 add nothing to the Dice sums, the CE (mean over the valid pixels of the local batch, 0 when there are none, as the
-reference skips it) or the validation counts, and their gradient is exactly 0.  It runs the split entry points
-(b2u_dice_ce_ign_*), with the same data-parallel batch Dice; the CE weight 1 / #valid stays on the device.
+reference skips it) or the validation counts, and their gradient is exactly 0.  It runs the same entry points with the
+kernels' ignore-label variant, with the same data-parallel batch Dice; the CE weight 1 / #valid stays on the device.
 
 Not covered (raise): an ignore label with `do_bg=True`.  The ignore-label loss covers the configuration the reference
 trainer builds for label maps (Dice without the background class, nnUNetTrainer.py:363-365), as the region loss covers
@@ -52,40 +52,6 @@ def _prep(logits: torch.Tensor, target: torch.Tensor):
     return logits.float().contiguous(), target.contiguous(), B, C, plane
 
 
-class _DiceCE(Function):
-    @staticmethod
-    def forward(ctx, logits, target, weight_ce, weight_dice, batch_dice, do_bg, smooth):
-        z, t, B, C, plane = _prep(logits, target)
-        lib = L.load()
-        dev = z.device
-        work = torch.empty(int(lib.b2u_dice_ce_work_doubles(B, C, plane)), dtype=torch.float64, device=dev)
-        out3 = torch.empty(3, dtype=torch.float32, device=dev)
-        counts = torch.empty((3, C), dtype=torch.int64, device=dev)
-        bad = torch.zeros(1, dtype=torch.int32, device=dev)
-        with torch.cuda.device(dev):
-            L.check(lib.b2u_dice_ce_forward(z.data_ptr(), t.data_ptr(), _KIND[t.dtype], work.data_ptr(), out3.data_ptr(),
-                                            counts.data_ptr(), bad.data_ptr(), B, C, plane, float(weight_ce),
-                                            float(weight_dice), int(batch_dice), int(do_bg), float(smooth),
-                                            torch.cuda.current_stream(dev).cuda_stream), "dice_ce_forward")
-        ctx.save_for_backward(z, t, work)
-        ctx.cfg = (B, C, plane, float(weight_ce), float(weight_dice), int(batch_dice), int(do_bg), float(smooth))
-        ctx.in_dtype, ctx.in_shape = logits.dtype, logits.shape
-        ctx.mark_non_differentiable(out3, counts, bad)
-        return out3[0].clone(), out3, counts, bad
-
-    @staticmethod
-    def backward(ctx, g, *_unused):
-        z, t, work = ctx.saved_tensors
-        B, C, plane, wce, wdc, bd, bg, smooth = ctx.cfg
-        grad = torch.empty_like(z)
-        with torch.cuda.device(z.device):
-            L.check(L.load().b2u_dice_ce_backward(z.data_ptr(), t.data_ptr(), _KIND[t.dtype], work.data_ptr(),
-                                                  grad.data_ptr(), B, C, plane, wce, wdc, bd, bg, smooth, 1.0,
-                                                  torch.cuda.current_stream(z.device).cuda_stream), "dice_ce_backward")
-        grad = (grad * g).view(ctx.in_shape).to(ctx.in_dtype)
-        return grad, None, None, None, None, None, None
-
-
 def _ddp_batch_dice(batch_dice: bool, ddp: bool) -> bool:
     """True when the batch Dice sums are summed across ranks (dice.py:106: batch_dice and ddp, under DDP)."""
     dist = torch.distributed
@@ -100,94 +66,6 @@ def _grad_scales(g: torch.Tensor, all_reduce: bool):
     total = local.clone()
     torch.distributed.all_reduce(total)
     return local, total
-
-
-class _DiceCEAllReduced(Function):
-    """Dice + CE whose batch Dice sums are all-reduced across the data-parallel ranks."""
-
-    @staticmethod
-    def forward(ctx, logits, target, weight_ce, weight_dice, do_bg, smooth):
-        z, t, B, C, plane = _prep(logits, target)
-        lib = L.load()
-        dev = z.device
-        work = torch.empty(int(lib.b2u_dice_ce_work_doubles(B, C, plane)), dtype=torch.float64, device=dev)
-        bsum = torch.empty((C, 3), dtype=torch.float64, device=dev)
-        out3 = torch.empty(3, dtype=torch.float32, device=dev)
-        counts = torch.empty((3, C), dtype=torch.int64, device=dev)
-        bad = torch.zeros(1, dtype=torch.int32, device=dev)
-        with torch.cuda.device(dev):
-            L.check(lib.b2u_dice_ce_stats(z.data_ptr(), t.data_ptr(), _KIND[t.dtype], work.data_ptr(), bsum.data_ptr(),
-                                          bad.data_ptr(), B, C, plane, torch.cuda.current_stream(dev).cuda_stream),
-                    "dice_ce_stats")
-            torch.distributed.all_reduce(bsum)
-            L.check(lib.b2u_dice_ce_finalize(work.data_ptr(), bsum.data_ptr(), out3.data_ptr(), counts.data_ptr(), B, C,
-                                             plane, float(weight_ce), float(weight_dice), 1, int(do_bg), float(smooth),
-                                             torch.cuda.current_stream(dev).cuda_stream), "dice_ce_finalize")
-        ctx.save_for_backward(z, t, work, bsum)
-        ctx.cfg = (B, C, plane, float(weight_ce), float(weight_dice), int(do_bg), float(smooth))
-        ctx.in_dtype, ctx.in_shape = logits.dtype, logits.shape
-        ctx.mark_non_differentiable(out3, counts, bad)
-        return out3[0].clone(), out3, counts, bad
-
-    @staticmethod
-    def backward(ctx, g, *_unused):
-        z, t, work, bsum = ctx.saved_tensors
-        B, C, plane, wce, wdc, bg, smooth = ctx.cfg
-        local, total = _grad_scales(g, all_reduce=True)
-        grad = torch.empty_like(z)
-        with torch.cuda.device(z.device):
-            L.check(L.load().b2u_dice_ce_backward_scaled(z.data_ptr(), t.data_ptr(), _KIND[t.dtype], work.data_ptr(),
-                                                         bsum.data_ptr(), grad.data_ptr(), B, C, plane, wce, wdc, 1, bg,
-                                                         smooth, local.data_ptr(), total.data_ptr(),
-                                                         torch.cuda.current_stream(z.device).cuda_stream),
-                    "dice_ce_backward_scaled")
-        return grad.view(ctx.in_shape).to(ctx.in_dtype), None, None, None, None, None
-
-
-class _DiceCEIgnore(Function):
-    """Dice + CE over the pixels whose label is not `ignore_label` (compound_losses.py:38-53); the batch Dice sums are
-    all-reduced across the data-parallel ranks when `all_reduce`."""
-
-    @staticmethod
-    def forward(ctx, logits, target, ignore_label, weight_ce, weight_dice, batch_dice, do_bg, smooth, all_reduce):
-        z, t, B, C, plane = _prep(logits, target)
-        lib = L.load()
-        dev = z.device
-        work = torch.empty(int(lib.b2u_dice_ce_ign_work_doubles(B, C, plane)), dtype=torch.float64, device=dev)
-        bsum = torch.empty((C, 3), dtype=torch.float64, device=dev)
-        out3 = torch.empty(3, dtype=torch.float32, device=dev)
-        counts = torch.empty((3, C), dtype=torch.int64, device=dev)
-        bad = torch.zeros(1, dtype=torch.int32, device=dev)
-        with torch.cuda.device(dev):
-            L.check(lib.b2u_dice_ce_ign_stats(z.data_ptr(), t.data_ptr(), _KIND[t.dtype], ignore_label, work.data_ptr(),
-                                              bsum.data_ptr(), bad.data_ptr(), B, C, plane,
-                                              torch.cuda.current_stream(dev).cuda_stream), "dice_ce_ign_stats")
-            if all_reduce:
-                torch.distributed.all_reduce(bsum)
-            L.check(lib.b2u_dice_ce_ign_finalize(work.data_ptr(), bsum.data_ptr(), out3.data_ptr(), counts.data_ptr(), B,
-                                                 C, plane, float(weight_ce), float(weight_dice), int(batch_dice),
-                                                 int(do_bg), float(smooth), torch.cuda.current_stream(dev).cuda_stream),
-                    "dice_ce_ign_finalize")
-        ctx.save_for_backward(z, t, work, bsum)
-        ctx.cfg = (ignore_label, B, C, plane, float(weight_ce), float(weight_dice), int(batch_dice), int(do_bg),
-                   float(smooth), bool(all_reduce))
-        ctx.in_dtype, ctx.in_shape = logits.dtype, logits.shape
-        ctx.mark_non_differentiable(out3, counts, bad)
-        return out3[0].clone(), out3, counts, bad
-
-    @staticmethod
-    def backward(ctx, g, *_unused):
-        z, t, work, bsum = ctx.saved_tensors
-        ign, B, C, plane, wce, wdc, bd, bg, smooth, all_reduce = ctx.cfg
-        local, total = _grad_scales(g, all_reduce)
-        grad = torch.empty_like(z)
-        with torch.cuda.device(z.device):
-            L.check(L.load().b2u_dice_ce_ign_backward(z.data_ptr(), t.data_ptr(), _KIND[t.dtype], ign, work.data_ptr(),
-                                                      bsum.data_ptr(), grad.data_ptr(), B, C, plane, wce, wdc, bd, bg,
-                                                      smooth, local.data_ptr(), total.data_ptr(),
-                                                      torch.cuda.current_stream(z.device).cuda_stream),
-                    "dice_ce_ign_backward")
-        return grad.view(ctx.in_shape).to(ctx.in_dtype), None, None, None, None, None, None, None, None
 
 
 def _prep_regions(logits: torch.Tensor, target: torch.Tensor, has_ignore: bool):
@@ -207,45 +85,111 @@ def _prep_regions(logits: torch.Tensor, target: torch.Tensor, has_ignore: bool):
     return logits.float().contiguous(), target.contiguous(), B, R, plane
 
 
-class _DiceBCE(Function):
+def _ptr(x):
+    return None if x is None else x.data_ptr()   # None: NULL
+
+
+class _LabelMaps:
+    """Softmax Dice + CE on label maps (b2u_dice_ce_*), with or without an ignore label."""
+    name, counts_dtype, has_bad_label = "dice_ce", torch.int64, True
+
+    def __init__(self, m: "DC_and_CE_loss"):
+        self.all_reduce = _ddp_batch_dice(m.batch_dice, m.ddp)
+        self.ign = int(m.ignore_label is not None)
+        self.label = m.ignore_label if self.ign else 0
+        self.batch_sums = self.all_reduce   # else NULL: finalize and backward sum the per-sample records in work
+        self.cfg = (float(m.weight_ce), float(m.weight_dice), int(m.batch_dice), int(m.do_bg), float(m.smooth))
+        # without an ignore label or an all-reduce the kernel runs unscaled and the incoming gradient is applied in torch
+        self.device_scales = bool(self.ign or self.all_reduce)
+
+    def prep(self, logits, target):
+        return _prep(logits, target)
+
+    def work_doubles(self, B, C, plane):
+        return L.load().b2u_dice_ce_work_doubles(B, C, plane, self.ign)
+
+    def stats(self, z, t, work, bsum, bad, B, C, plane, s):
+        return L.load().b2u_dice_ce_stats(z.data_ptr(), t.data_ptr(), _KIND[t.dtype], self.ign, self.label,
+                                          work.data_ptr(), _ptr(bsum), bad.data_ptr(), B, C, plane, s)
+
+    def finalize(self, work, bsum, out3, counts, B, C, plane, s):
+        return L.load().b2u_dice_ce_finalize(work.data_ptr(), _ptr(bsum), out3.data_ptr(), counts.data_ptr(), B, C,
+                                             plane, self.ign, *self.cfg, s)
+
+    def backward(self, z, t, work, bsum, grad, ce_scale, dice_scale, B, C, plane, s):
+        return L.load().b2u_dice_ce_backward(z.data_ptr(), t.data_ptr(), _KIND[t.dtype], self.ign, self.label,
+                                             work.data_ptr(), _ptr(bsum), grad.data_ptr(), B, C, plane, *self.cfg,
+                                             _ptr(ce_scale), _ptr(dice_scale), s)
+
+
+class _Regions:
+    """Sigmoid Dice + BCE on region targets (b2u_dice_bce_*), with or without an ignore channel."""
+    name, counts_dtype, has_bad_label, device_scales = "dice_bce", torch.float32, False, True
+    batch_sums = True                       # the region kernels take the batch Dice from the batch sums only
+
+    def __init__(self, m: "DC_and_BCE_loss"):
+        self.all_reduce = _ddp_batch_dice(m.batch_dice, m.ddp)
+        self.ign = int(m.use_ignore_label)
+        self.w = (float(m.weight_ce), float(m.weight_dice), int(m.batch_dice))
+        self.smooth = float(m.smooth)
+
+    def prep(self, logits, target):
+        return _prep_regions(logits, target, self.ign)
+
+    def work_doubles(self, B, R, plane):
+        return L.load().b2u_dice_bce_work_doubles(B, R, plane)
+
+    def stats(self, z, t, work, bsum, bad, B, R, plane, s):
+        return L.load().b2u_dice_bce_stats(z.data_ptr(), t.data_ptr(), _KIND[t.dtype], self.ign, work.data_ptr(),
+                                           _ptr(bsum), B, R, plane, s)
+
+    def finalize(self, work, bsum, out3, counts, B, R, plane, s):
+        return L.load().b2u_dice_bce_finalize(work.data_ptr(), _ptr(bsum), out3.data_ptr(), counts.data_ptr(), B, R,
+                                              plane, *self.w, self.ign, self.smooth, s)
+
+    def backward(self, z, t, work, bsum, grad, ce_scale, dice_scale, B, R, plane, s):
+        return L.load().b2u_dice_bce_backward(z.data_ptr(), t.data_ptr(), _KIND[t.dtype], self.ign, work.data_ptr(),
+                                              _ptr(bsum), grad.data_ptr(), B, R, plane, *self.w, self.smooth,
+                                              _ptr(ce_scale), _ptr(dice_scale), s)
+
+
+class _FusedLoss(Function):
+    """Statistics pass, all-reduce of the batch Dice sums across ranks (`fam.all_reduce`), finalisation; the gradient
+    pass in backward.  `fam` (_LabelMaps, _Regions) binds its family's entry points to the loss's configuration."""
+
     @staticmethod
-    def forward(ctx, logits, target, weight_ce, weight_dice, batch_dice, has_ignore, smooth, all_reduce):
-        z, t, B, R, plane = _prep_regions(logits, target, has_ignore)
-        lib = L.load()
+    def forward(ctx, logits, target, fam):
+        z, t, B, n, plane = fam.prep(logits, target)
         dev = z.device
-        work = torch.empty(int(lib.b2u_dice_bce_work_doubles(B, R, plane)), dtype=torch.float64, device=dev)
-        bsum = torch.empty((R, 3), dtype=torch.float64, device=dev)
+        work = torch.empty(int(fam.work_doubles(B, n, plane)), dtype=torch.float64, device=dev)
+        bsum = torch.empty((n, 3), dtype=torch.float64, device=dev) if fam.batch_sums else None
         out3 = torch.empty(3, dtype=torch.float32, device=dev)
-        counts = torch.empty((3, R), dtype=torch.float32, device=dev)
+        counts = torch.empty((3, n), dtype=fam.counts_dtype, device=dev)
+        bad = torch.zeros(1, dtype=torch.int32, device=dev) if fam.has_bad_label else None
         with torch.cuda.device(dev):
-            L.check(lib.b2u_dice_bce_stats(z.data_ptr(), t.data_ptr(), _KIND[t.dtype], int(has_ignore), work.data_ptr(),
-                                           bsum.data_ptr(), B, R, plane, torch.cuda.current_stream(dev).cuda_stream),
-                    "dice_bce_stats")
-            if all_reduce:
+            s = torch.cuda.current_stream(dev).cuda_stream
+            L.check(fam.stats(z, t, work, bsum, bad, B, n, plane, s), fam.name + "_stats")
+            if fam.all_reduce:
                 torch.distributed.all_reduce(bsum)
-            L.check(lib.b2u_dice_bce_finalize(work.data_ptr(), bsum.data_ptr(), out3.data_ptr(), counts.data_ptr(), B, R,
-                                              plane, float(weight_ce), float(weight_dice), int(batch_dice),
-                                              int(has_ignore), float(smooth), torch.cuda.current_stream(dev).cuda_stream),
-                    "dice_bce_finalize")
+            L.check(fam.finalize(work, bsum, out3, counts, B, n, plane, s), fam.name + "_finalize")
         ctx.save_for_backward(z, t, work, bsum)
-        ctx.cfg = (B, R, plane, float(weight_ce), float(weight_dice), int(batch_dice), int(has_ignore), float(smooth),
-                   bool(all_reduce))
+        ctx.fam, ctx.dims = fam, (B, n, plane)
         ctx.in_dtype, ctx.in_shape = logits.dtype, logits.shape
-        ctx.mark_non_differentiable(out3, counts)
-        return out3[0].clone(), out3, counts
+        ctx.mark_non_differentiable(*(x for x in (out3, counts, bad) if x is not None))
+        return out3[0].clone(), out3, counts, bad
 
     @staticmethod
     def backward(ctx, g, *_unused):
         z, t, work, bsum = ctx.saved_tensors
-        B, R, plane, wce, wdc, bd, ign, smooth, all_reduce = ctx.cfg
-        local, total = _grad_scales(g, all_reduce)
+        fam = ctx.fam
+        scales = _grad_scales(g, fam.all_reduce) if fam.device_scales else (None, None)
         grad = torch.empty_like(z)
         with torch.cuda.device(z.device):
-            L.check(L.load().b2u_dice_bce_backward(z.data_ptr(), t.data_ptr(), _KIND[t.dtype], ign, work.data_ptr(),
-                                                   bsum.data_ptr(), grad.data_ptr(), B, R, plane, wce, wdc, bd, smooth,
-                                                   local.data_ptr(), total.data_ptr(),
-                                                   torch.cuda.current_stream(z.device).cuda_stream), "dice_bce_backward")
-        return grad.view(ctx.in_shape).to(ctx.in_dtype), None, None, None, None, None, None, None
+            L.check(fam.backward(z, t, work, bsum, grad, *scales, *ctx.dims,
+                                 torch.cuda.current_stream(z.device).cuda_stream), fam.name + "_backward")
+        if not fam.device_scales:
+            grad = grad * g
+        return grad.view(ctx.in_shape).to(ctx.in_dtype), None, None
 
 
 class DC_and_CE_loss(nn.Module):
@@ -276,16 +220,7 @@ class DC_and_CE_loss(nn.Module):
         self.check_labels = False
 
     def _run(self, net_output, target):
-        if self.ignore_label is not None:
-            loss, out3, counts, bad = _DiceCEIgnore.apply(net_output, target, self.ignore_label, self.weight_ce,
-                                                          self.weight_dice, self.batch_dice, self.do_bg, self.smooth,
-                                                          _ddp_batch_dice(self.batch_dice, self.ddp))
-        elif _ddp_batch_dice(self.batch_dice, self.ddp):
-            loss, out3, counts, bad = _DiceCEAllReduced.apply(net_output, target, self.weight_ce, self.weight_dice,
-                                                              self.do_bg, self.smooth)
-        else:
-            loss, out3, counts, bad = _DiceCE.apply(net_output, target, self.weight_ce, self.weight_dice,
-                                                    self.batch_dice, self.do_bg, self.smooth)
+        loss, out3, counts, bad = _FusedLoss.apply(net_output, target, _LabelMaps(self))
         if self.check_labels and int(bad.item()):
             raise RuntimeError("target contains labels outside [0, num_classes)")
         return loss, out3, counts, bad
@@ -318,10 +253,7 @@ class DC_and_BCE_loss(nn.Module):
         self.use_ignore_label = bool(use_ignore_label)
 
     def _run(self, net_output, target):
-        loss, out3, counts = _DiceBCE.apply(net_output, target, self.weight_ce, self.weight_dice, self.batch_dice,
-                                            self.use_ignore_label, self.smooth,
-                                            _ddp_batch_dice(self.batch_dice, self.ddp))
-        return loss, out3, counts, None
+        return _FusedLoss.apply(net_output, target, _Regions(self))
 
     def forward(self, net_output: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
         return self._run(net_output, target)[0]

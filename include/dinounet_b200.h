@@ -279,73 +279,46 @@ int b2u_eval_sum_f64(const double* x, int64_t n, double* work, b2u_stream_t stre
 /* ---- Dice + cross-entropy loss and online-validation statistics on the logits of the forward path
  * (training/loss/compound_losses.py:31-56 `DC_and_CE_loss`, dice.py:72-119 `MemoryEfficientSoftDiceLoss`,
  * robust_ce_loss.py:12-16, built at nnUNetTrainer.py:363-365; consumer nnUNetTrainer.py:961-1005 `validation_step`).
- * logits fp32 [B, C, plane] (plane = H*W); target [B, plane] labels, target_kind 0 = uint8, 1 = int32, 2 = int64,
- * 3 = float32 (nnU-Net hands float label maps).  work: caller-owned, b2u_dice_ce_work_doubles(B, C, plane) doubles.
- * forward: out3[0] = weight_ce*CE + weight_dice*dice, out3[1] = CE (mean over all pixels), out3[2] = dice term
- *   (-mean_c (2*sum(p*y)+smooth)/max(sum(y)+sum(p)+smooth, 1e-8); over the batch if batch_dice, background class skipped
- *   unless do_bg);  tp_fp_fn (optional) int64 [3][C] = hard tp / fp / fn of argmax(logits) vs target, summed over the
- *   batch (get_tp_fp_fn_tn with axes (0,2,3), nnUNetTrainer.py:971-991);  *bad_label is set to 1 if a label is outside
- *   [0, C) (torch raises a device assert there).  Deterministic (fixed reduction order, fp64 partials).
- * backward: grad_logits fp32 [B, C, plane] = grad_scale * dLoss/dlogits, from the sums the forward left in `work`.
- * 2 <= C <= 32.  An ignore label takes the b2u_dice_ce_ign_* family below.
- *
- * Split forward for data-parallel batch Dice (dice.py:106-110, AllGatherGrad): b2u_dice_ce_stats runs the statistics
- * pass and writes batch_sums fp64 [C][3] = (intersect, sum_pred, sum_gt) of every class summed over the local batch;
- * the caller may all-reduce batch_sums across ranks; b2u_dice_ce_finalize then forms out3 / tp_fp_fn as the fused
- * forward does, with the batch Dice taken from batch_sums (batch_dice = 0 ignores them: per-sample Dice stays local).
- * b2u_dice_ce_backward_scaled: grad = *ce_scale * dCE/dlogits + *dice_scale * d(dice term)/dlogits (device scalars: the
- * local incoming gradient and its sum over ranks), Dice coefficients from batch_sums. */
-int64_t b2u_dice_ce_work_doubles(int32_t B, int32_t C, int64_t plane);
-int b2u_dice_ce_forward(const float* logits, const void* target, int32_t target_kind, double* work, float* out3,
-                        int64_t* tp_fp_fn, int32_t* bad_label, int32_t B, int32_t C, int64_t plane, float weight_ce,
-                        float weight_dice, int32_t batch_dice, int32_t do_bg, float smooth, b2u_stream_t stream);
-int b2u_dice_ce_backward(const float* logits, const void* target, int32_t target_kind, const double* work,
-                         float* grad_logits, int32_t B, int32_t C, int64_t plane, float weight_ce, float weight_dice,
-                         int32_t batch_dice, int32_t do_bg, float smooth, float grad_scale, b2u_stream_t stream);
-int b2u_dice_ce_stats(const float* logits, const void* target, int32_t target_kind, double* work, double* batch_sums,
-                      int32_t* bad_label, int32_t B, int32_t C, int64_t plane, b2u_stream_t stream);
+ * logits fp32 [B, C, plane] (plane = H*W), 2 <= C <= 32; target [B, plane] labels, target_kind 0 = uint8, 1 = int32,
+ * 2 = int64, 3 = float32 (nnU-Net hands float label maps).  has_ignore: a pixel labelled ignore_label (any integer;
+ * nnU-Net uses C) counts for nothing (compound_losses.py:21-22, 38-53; validation_step's mask, nnUNetTrainer.py:982-986);
+ * without it ignore_label is not read.  work: caller-owned, b2u_dice_ce_work_doubles(B, C, plane, has_ignore) doubles,
+ * shared by the three calls.  Deterministic (fixed reduction order, fp64 partials).
+ * stats: one pass over logits and target;  *bad_label = 1 if a (valid) label is outside [0, C) (torch raises a device
+ *   assert there);  batch_sums (NULL: not needed) fp64 [C][3] = (intersect, sum_pred, sum_gt) of every class over the
+ *   valid pixels of the local batch, for the caller to all-reduce across data-parallel ranks (dice.py:106-110,
+ *   AllGatherGrad) before the finalisation.
+ * finalize: out3[0] = weight_ce*CE + weight_dice*dice, out3[1] = CE (mean over the valid pixels; 0 when there are none,
+ *   as the reference skips it), out3[2] = dice term (-mean_c (2*sum(p*y)+smooth)/max(sum(y)+sum(p)+smooth, 1e-8); over
+ *   the batch if batch_dice, background class skipped unless do_bg);  tp_fp_fn (optional) int64 [3][C] = hard tp / fp / fn
+ *   of argmax(logits) vs target over the valid pixels, summed over the batch (get_tp_fp_fn_tn with axes (0,2,3)).
+ * backward: grad_logits fp32 [B, C, plane] = *ce_scale * dCE/dlogits + *dice_scale * d(dice term)/dlogits, exactly 0 at
+ *   ignored pixels.  ce_scale, dice_scale: device scalars (NULL: 1), e.g. the local incoming gradient and its sum over
+ *   ranks (the backward of AllGatherGrad, ddp_allgather.py:43-48).
+ * finalize and backward take the batch Dice from batch_sums when given (batch_dice = 0 ignores them: per-sample Dice
+ * stays local), else from the per-sample sums in work, with the same result bits. */
+int64_t b2u_dice_ce_work_doubles(int32_t B, int32_t C, int64_t plane, int32_t has_ignore);
+int b2u_dice_ce_stats(const float* logits, const void* target, int32_t target_kind, int32_t has_ignore,
+                      int32_t ignore_label, double* work, double* batch_sums, int32_t* bad_label, int32_t B, int32_t C,
+                      int64_t plane, b2u_stream_t stream);
 int b2u_dice_ce_finalize(double* work, const double* batch_sums, float* out3, int64_t* tp_fp_fn, int32_t B, int32_t C,
-                         int64_t plane, float weight_ce, float weight_dice, int32_t batch_dice, int32_t do_bg,
-                         float smooth, b2u_stream_t stream);
-int b2u_dice_ce_backward_scaled(const float* logits, const void* target, int32_t target_kind, const double* work,
-                                const double* batch_sums, float* grad_logits, int32_t B, int32_t C, int64_t plane,
-                                float weight_ce, float weight_dice, int32_t batch_dice, int32_t do_bg, float smooth,
-                                const float* ce_scale, const float* dice_scale, b2u_stream_t stream);
-
-/* ---- The same loss with an ignore label (DC_and_CE_loss(..., ignore_label), compound_losses.py:21-22, 38-53;
- * validation_step's label-map mask, nnUNetTrainer.py:982-986).  A pixel whose label equals ignore_label (any integer;
- * nnU-Net uses C) is ignored; the others are valid.  work: b2u_dice_ce_ign_work_doubles(B, C, plane) doubles; the
- * per-sample records also hold the valid-pixel count.
- * stats: one pass; batch_sums fp64 [C][3] = (intersect, sum_pred, sum_gt) over the valid pixels, summed over the batch
- *   (all-reducible as above); *bad_label = 1 if a valid pixel's label is outside [0, C).
- * finalize: out3[1] = CE summed over the valid pixels / their number (0 when the batch has none: the reference skips
- *   the CE), out3[2] = the dice term over the valid pixels (batch Dice from batch_sums when batch_dice), out3[0] =
- *   weight_ce*CE + weight_dice*dice;  tp_fp_fn (optional) int64 [3][C] = hard counts over the valid pixels only.
- * backward: grad = *ce_scale * dCE/dlogits + *dice_scale * d(dice term)/dlogits, exactly 0 at ignored pixels; the CE
- *   weight weight_ce / #valid is formed on the device.  Deterministic (fixed reduction order, fp64 partials). */
-int64_t b2u_dice_ce_ign_work_doubles(int32_t B, int32_t C, int64_t plane);
-int b2u_dice_ce_ign_stats(const float* logits, const void* target, int32_t target_kind, int32_t ignore_label,
-                          double* work, double* batch_sums, int32_t* bad_label, int32_t B, int32_t C, int64_t plane,
-                          b2u_stream_t stream);
-int b2u_dice_ce_ign_finalize(double* work, const double* batch_sums, float* out3, int64_t* tp_fp_fn, int32_t B,
-                             int32_t C, int64_t plane, float weight_ce, float weight_dice, int32_t batch_dice,
-                             int32_t do_bg, float smooth, b2u_stream_t stream);
-int b2u_dice_ce_ign_backward(const float* logits, const void* target, int32_t target_kind, int32_t ignore_label,
-                             const double* work, const double* batch_sums, float* grad_logits, int32_t B, int32_t C,
-                             int64_t plane, float weight_ce, float weight_dice, int32_t batch_dice, int32_t do_bg,
-                             float smooth, const float* ce_scale, const float* dice_scale, b2u_stream_t stream);
+                         int64_t plane, int32_t has_ignore, float weight_ce, float weight_dice, int32_t batch_dice,
+                         int32_t do_bg, float smooth, b2u_stream_t stream);
+int b2u_dice_ce_backward(const float* logits, const void* target, int32_t target_kind, int32_t has_ignore,
+                         int32_t ignore_label, const double* work, const double* batch_sums, float* grad_logits,
+                         int32_t B, int32_t C, int64_t plane, float weight_ce, float weight_dice, int32_t batch_dice,
+                         int32_t do_bg, float smooth, const float* ce_scale, const float* dice_scale,
+                         b2u_stream_t stream);
 
 /* ---- Region-based Dice + BCE (compound_losses.py:59-99 `DC_and_BCE_loss` with MemoryEfficientSoftDiceLoss on
  * sigmoid(logits), do_bg, built at nnUNetTrainer.py:356-361; validation_step's region branch :973-994).
  * logits fp32 [B, R, plane], 1 <= R <= 32; target [B, R + has_ignore, plane] of target_kind (as above), used as real
  * values; with has_ignore the last channel is the ignore channel: a pixel is valid where (1 - t_ign) != 0.
- * work: b2u_dice_bce_work_doubles(B, R, plane) doubles.  Same split as the softmax loss:
- * stats: one pass; batch_sums fp64 [R][3] = (intersect, sum_pred, sum_gt) over valid pixels, summed over the batch.
- * finalize: out3[0] = weight_ce*BCE + weight_dice*dice, out3[1] = BCE (mean over B*R*plane; with has_ignore
- *   sum(bce * valid) / max(#valid pixels, 1e-8)), out3[2] = -mean_r (2I+smooth)/max(G+P+smooth, 1e-8) (batch Dice from
- *   batch_sums, else per sample);  tp_fp_fn (optional) float [3][R] = sum over the batch of pred*y*w, pred*(1-y)*w,
- *   (1-pred)*y*w with pred = sigmoid(z) > 0.5 and w = 1 - t_ign (1 without an ignore channel).
- * backward: grad = *ce_scale * dBCE/dlogits + *dice_scale * d(dice term)/dlogits.  Deterministic. */
+ * work: b2u_dice_bce_work_doubles(B, R, plane) doubles.  The same three calls as the label maps, except that batch_sums
+ * fp64 [R][3] is required: the batch Dice comes from it only.  finalize: out3[1] = BCE (mean over B*R*plane; with has_ignore sum(bce * valid) / max(#valid pixels, 1e-8)),
+ * out3[2] = -mean_r (2I+smooth)/max(G+P+smooth, 1e-8);  tp_fp_fn (optional) float [3][R] = sum over the batch of
+ * pred*y*w, pred*(1-y)*w, (1-pred)*y*w with pred = sigmoid(z) > 0.5 and w = 1 - t_ign (1 without an ignore channel).
+ * backward: grad = *ce_scale * dBCE/dlogits + *dice_scale * d(dice term)/dlogits (both scalars required). */
 int64_t b2u_dice_bce_work_doubles(int32_t B, int32_t R, int64_t plane);
 int b2u_dice_bce_stats(const float* logits, const void* target, int32_t target_kind, int32_t has_ignore, double* work,
                        double* batch_sums, int32_t B, int32_t R, int64_t plane, b2u_stream_t stream);

@@ -75,7 +75,7 @@ class _Recorder:
     def __getattr__(self, name):
         def fn(*a):
             self.calls.append((name, a))
-            return 0
+            return 64 if name.endswith("_work_doubles") else 0
         return fn
 
 
@@ -86,39 +86,74 @@ def rec(monkeypatch):
     r = _Recorder()
     monkeypatch.setattr(L, "load", lambda: r)
     # CPU tensors stand in for device buffers: the stand-in library never reads them
-    monkeypatch.setattr(LS, "_prep", lambda z, t: (z.float().contiguous(), t.contiguous(), z.shape[0], z.shape[1],
-                                                   int(np.prod(z.shape[2:]))))
+    prep = lambda z, t, *_: (z.float().contiguous(), t.contiguous(), z.shape[0], z.shape[1], int(np.prod(z.shape[2:])))
+    monkeypatch.setattr(LS, "_prep", prep)
+    monkeypatch.setattr(LS, "_prep_regions", prep)
     monkeypatch.setattr(torch.cuda, "device", lambda dev: contextlib.nullcontext())
     monkeypatch.setattr(torch.cuda, "current_stream", lambda dev=None: type("S", (), {"cuda_stream": 0})())
     return r
 
 
-def _fwd_bwd(mod):
+def _fwd_bwd(monkeypatch, regions, ignore, batch_dice, all_reduce):
+    """One forward + backward of the label-map loss (ignore label 3) or the region loss (ignore channel); with
+    `all_reduce`, as under data-parallel batch Dice (the all-reduce itself is the identity here)."""
+    from dinounet_b200 import loss as LS
+    if all_reduce:
+        monkeypatch.setattr(LS, "_ddp_batch_dice", lambda batch_dice, ddp: True)
+        monkeypatch.setattr(torch.distributed, "all_reduce", lambda t: None)
+    dice_kw = {"batch_dice": batch_dice, "smooth": 1e-5, "do_bg": regions, "ddp": all_reduce}
+    if regions:
+        mod, t = LS.DC_and_BCE_loss({}, dice_kw, use_ignore_label=ignore), torch.zeros(2, 3 + ignore, 8, 8)
+    else:
+        mod, t = LS.DC_and_CE_loss(dice_kw, {}, 1, 1, ignore_label=3 if ignore else None), torch.zeros(2, 1, 8, 8)
     z = torch.zeros(2, 3, 8, 8, requires_grad=True)
-    mod(z, torch.zeros(2, 1, 8, 8)).backward()
-    return z
+    mod(z, t).backward()
 
 
-@pytest.mark.parametrize("batch_dice", [False, True])
-def test_no_ignore_label_runs_todays_calls(rec, batch_dice):
-    from dinounet_b200.loss import DC_and_CE_loss
-    _fwd_bwd(DC_and_CE_loss({"batch_dice": batch_dice, "smooth": 1e-5, "do_bg": False, "ddp": False}, {}, 1, 1,
-                            ignore_label=None))
-    assert [n for n, _ in rec.calls] == ["b2u_dice_ce_work_doubles", "b2u_dice_ce_forward", "b2u_dice_ce_backward"]
+# argument positions in the (stats, finalize, backward) calls: work, batch_sums, and the has-ignore flag; batch_dice in
+# finalize and backward
+_POS = {"dice_ce": dict(work=(5, 0, 5), bsum=(6, 1, 6), ign=(3, 7, 3), batch_dice=(10, 13)),
+        "dice_bce": dict(work=(4, 0, 4), bsum=(5, 1, 5), ign=(3, 10, 3), batch_dice=(9, 12))}
 
 
-@pytest.mark.parametrize("batch_dice", [False, True])
-def test_ignore_label_runs_the_ignore_family(rec, batch_dice):
-    from dinounet_b200.loss import DC_and_CE_loss
-    _fwd_bwd(DC_and_CE_loss({"batch_dice": batch_dice, "smooth": 1e-5, "do_bg": False, "ddp": False}, {}, 1, 1,
-                            ignore_label=3))
-    names = [n for n, _ in rec.calls]
-    assert names == ["b2u_dice_ce_ign_work_doubles", "b2u_dice_ce_ign_stats", "b2u_dice_ce_ign_finalize",
-                     "b2u_dice_ce_ign_backward"]
-    stats, fin, bwd = (a for n, a in rec.calls[1:])
-    assert stats[3] == 3 and bwd[3] == 3                                   # the ignore label reaches both passes
-    assert stats[4] == fin[0] == bwd[4] and stats[5] == fin[1] == bwd[5]   # work and batch sums are shared
-    assert fin[9] == batch_dice and bwd[12] == batch_dice
+def _check_calls(rec, fam, ignore, batch_dice, all_reduce):
+    """The one call sequence of every configuration: one work buffer shared by the three calls; the batch sums NULL in
+    all three for label maps without an all-reduce, else one buffer shared by all three; batch_dice reaching finalize
+    and backward.  Returns the (stats, finalize, backward) arguments."""
+    assert [n for n, _ in rec.calls] == [f"b2u_{fam}_{s}" for s in ("work_doubles", "stats", "finalize", "backward")]
+    calls = [a for _, a in rec.calls[1:]]
+    pos = _POS[fam]
+    work = {a[i] for a, i in zip(calls, pos["work"])}
+    assert len(work) == 1 and None not in work and 0 not in work
+    bsum = [a[i] for a, i in zip(calls, pos["bsum"])]
+    assert bsum == [bsum[0]] * 3 and (bsum[0] is not None) == (all_reduce or fam == "dice_bce")
+    assert [a[i] for a, i in zip(calls, pos["ign"])] == [int(ignore)] * 3
+    (fin, bwd), (i_fin, i_bwd) = calls[1:], pos["batch_dice"]
+    assert fin[i_fin] == batch_dice and bwd[i_bwd] == batch_dice
+    return calls
+
+
+# batch_dice (the ids the label-map cases had when they took only that), the same under an all-reduce, the region loss
+_CASES = [pytest.param(False, False, False, id="False"), pytest.param(True, False, False, id="True"),
+          pytest.param(True, True, False, id="all_reduce"), pytest.param(False, False, True, id="regions-False"),
+          pytest.param(True, False, True, id="regions-True"), pytest.param(True, True, True, id="regions-all_reduce")]
+
+
+@pytest.mark.parametrize("batch_dice,all_reduce,regions", _CASES)
+def test_no_ignore_label_runs_todays_calls(rec, monkeypatch, batch_dice, all_reduce, regions):
+    _fwd_bwd(monkeypatch, regions, False, batch_dice, all_reduce)
+    bwd = _check_calls(rec, "dice_bce" if regions else "dice_ce", False, batch_dice, all_reduce)[2]
+    if not regions and not all_reduce:   # unit scales in the kernel; the incoming gradient is applied in torch
+        assert bwd[16] is None and bwd[17] is None
+
+
+@pytest.mark.parametrize("batch_dice,all_reduce,regions", _CASES)
+def test_ignore_label_runs_the_ignore_family(rec, monkeypatch, batch_dice, all_reduce, regions):
+    _fwd_bwd(monkeypatch, regions, True, batch_dice, all_reduce)
+    stats, _, bwd = _check_calls(rec, "dice_bce" if regions else "dice_ce", True, batch_dice, all_reduce)
+    if not regions:
+        assert stats[4] == 3 and bwd[4] == 3                               # the ignore label reaches both passes
+    assert bwd[-3] is not None and bwd[-2] is not None                     # the scales come from the device
 
 
 # ---- argument contract and the trainer
