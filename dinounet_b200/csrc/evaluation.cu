@@ -1,8 +1,8 @@
 // Scoring predictions against the ground truth on the device (reference: evaluation/evaluate_predictions.py:152-230
 // `compute_metrics`, with medpy's hd95 / asd: `__surface_distances`).
 //
-//   b2u_eval_masks  one pass over the two label volumes per label or region: the masks `seg == r` (numpy's `==`:
-//                   exact for integer dtypes, the label rounded to float32 for float32 volumes), their face-connectivity
+//   b2u_eval_masks  one pass over the two label volumes per label or region: the masks `seg == r` (numpy's `==`,
+//                   label_compare.cuh: exact for integer dtypes, the label rounded to float32 for float32 volumes), their face-connectivity
 //                   borders x ^ binary_erosion(x) with out-of-range neighbours 0 (scipy's border_value), and the exact
 //                   int64 TP / FP / FN / TN over the voxels whose reference is not the ignore label, plus the two masks'
 //                   populations.  Block reduction, then one integer atomic per block and counter.
@@ -24,6 +24,7 @@
 #include "../../include/dinounet_b200.h"
 #include "gemm_common.h"
 #include "host_util.h"
+#include "label_compare.cuh"
 
 namespace b2u {
 
@@ -41,18 +42,6 @@ struct RegionLabels {
   long long ignore_v;
   float ignore_f;
 };
-
-// dtype codes: B2U_EVAL_U8, _I8, _I16, _U16, _I32, _F32.  Integer values compare exactly as int64.
-__device__ __forceinline__ bool equals(const void* p, int dtype, long long i, long long v, float f) {
-  switch (dtype) {
-    case B2U_EVAL_U8: return static_cast<const uint8_t*>(p)[i] == v;
-    case B2U_EVAL_I8: return static_cast<const int8_t*>(p)[i] == v;
-    case B2U_EVAL_I16: return static_cast<const int16_t*>(p)[i] == v;
-    case B2U_EVAL_U16: return static_cast<const uint16_t*>(p)[i] == v;
-    case B2U_EVAL_I32: return static_cast<const int32_t*>(p)[i] == v;
-    default: return static_cast<const float*>(p)[i] == f;
-  }
-}
 
 __device__ __forceinline__ bool in_region(const void* p, int dtype, long long i, const RegionLabels& L) {
   bool m = false;
@@ -268,12 +257,12 @@ extern "C" int b2u_eval_masks(const void* ref, int32_t ref_dtype, const void* pr
   RegionLabels L{};
   for (int j = 0; j < n_labels; ++j) {
     L.v[j] = labels[j];
-    L.f[j] = static_cast<float>(labels[j]);
+    L.f[j] = label_as_f32(labels[j]);
   }
   L.n = n_labels;
   L.has_ignore = has_ignore != 0;
   L.ignore_v = ignore_label;
-  L.ignore_f = static_cast<float>(ignore_label);
+  L.ignore_f = label_as_f32(ignore_label);
   if (cudaMemsetAsync(counts, 0, 6 * sizeof(int64_t), stream) != cudaSuccess)
     return set_error(-1, "b2u_eval_masks: cudaMemsetAsync failed");
   const long long n = static_cast<long long>(Z) * Y * X;

@@ -240,6 +240,19 @@ def _score(reference_file, prediction_file, loaded, labels_or_regions, ignore_la
             "metrics": compute_metrics_arrays(seg_ref, seg_pred, labels_or_regions, ignore_label, spacing)}
 
 
+def read_ahead(n: int, read, num_processes: int):
+    """Yields read(0), ..., read(n - 1) in order while `num_processes` threads read the next cases."""
+    window = max(1, int(num_processes))
+    with ThreadPoolExecutor(window) as pool:
+        pending = [pool.submit(read, i) for i in range(min(window, n))]
+        for i in range(n):
+            loaded = pending[i].result()
+            if i + window < n:
+                pending.append(pool.submit(read, i + window))
+            pending[i] = None
+            yield loaded
+
+
 def compute_metrics(reference_file: str, prediction_file: str, image_reader_writer, labels_or_regions,
                     ignore_label: int = None) -> dict:
     """Drop-in for the reference's `compute_metrics`: reads both files with `image_reader_writer.read_seg` and scores
@@ -292,16 +305,45 @@ def aggregate(results: list, regions_or_labels) -> dict:
     return {"metric_per_case": results, "mean": means, "foreground_mean": foreground_mean}
 
 
-def save_summary_json(results: dict, output_file: str):
-    """The reference's `save_summary_json`: label / region keys as `str(key)`, written by `json` with indent 4 and
+def summary_text(results: dict) -> str:
+    """The text of the reference's `save_summary_json`: label / region keys as `str(key)`, `json` with indent 4 and
     sorted keys."""
     converted = deepcopy(results)
     converted["mean"] = {str(k): results["mean"][k] for k in results["mean"].keys()}
     for i in range(len(converted["metric_per_case"])):
         converted["metric_per_case"][i]["metrics"] = {str(k): v for k, v in
                                                       results["metric_per_case"][i]["metrics"].items()}
+    return json.dumps(converted, sort_keys=True, indent=4)
+
+
+def save_summary_json(results: dict, output_file: str):
+    """The reference's `save_summary_json`."""
     with open(output_file, "w") as f:
-        json.dump(converted, f, sort_keys=True, indent=4)
+        f.write(summary_text(results))
+
+
+def key_to_label_or_region(key: str):
+    """The reference's `key_to_label_or_region`: "3" -> 3, "(1, 2)" -> (1, 2)."""
+    try:
+        return int(key)
+    except ValueError:
+        key = key.replace("(", "").replace(")", "")
+        return tuple(int(i) for i in key.split(",") if len(i) > 0)
+
+
+def summary_keys_from_json(results: dict) -> dict:
+    """In place, what the reference's `load_summary_json` does after `load_json`: the label / region keys of `mean` and
+    of every case's `metrics` back to ints and tuples."""
+    results["mean"] = {key_to_label_or_region(k): results["mean"][k] for k in results["mean"].keys()}
+    for case in results["metric_per_case"]:
+        case["metrics"] = {key_to_label_or_region(k): case["metrics"][k] for k in case["metrics"].keys()}
+    return results
+
+
+def load_summary_json(filename: str) -> dict:
+    """The reference's `load_summary_json`: a summary written by `save_summary_json`, with its keys converted back."""
+    with open(filename) as f:
+        return summary_keys_from_json(json.load(f))
 
 
 def compute_metrics_on_folder(folder_ref: str, folder_pred: str, output_file: str, image_reader_writer,
@@ -326,16 +368,8 @@ def compute_metrics_on_folder(folder_ref: str, folder_pred: str, output_file: st
     def read(i):
         return image_reader_writer.read_seg(files_ref[i]), image_reader_writer.read_seg(files_pred[i])
 
-    window = max(1, int(num_processes))
-    results = []
-    with ThreadPoolExecutor(window) as pool:
-        pending = [pool.submit(read, i) for i in range(min(window, len(files_pred)))]
-        for i in range(len(files_pred)):
-            loaded = pending[i].result()
-            if i + window < len(files_pred):
-                pending.append(pool.submit(read, i + window))
-            pending[i] = None
-            results.append(_score(files_ref[i], files_pred[i], loaded, regions_or_labels, ignore_label))
+    results = [_score(files_ref[i], files_pred[i], loaded, regions_or_labels, ignore_label)
+               for i, loaded in enumerate(read_ahead(len(files_pred), read, num_processes))]
     result = aggregate(results, regions_or_labels)
     if output_file is not None:
         save_summary_json(result, output_file)

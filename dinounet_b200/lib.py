@@ -105,6 +105,7 @@ SIGNATURES = {
     "b2u_eval_masks": [vp, i32, vp, i32, i32, i32, i32, i32, C.POINTER(C.c_int64), i32, i32, i64, vp, vp, vp, vp],
     "b2u_eval_edt": [vp, i32, i32, i32, C.c_double, C.c_double, C.c_double, vp, vp, vp, vp],
     "b2u_eval_sum_f64": [vp, i64, vp, vp],
+    "b2u_pp_largest_component": [vp, i32, i32, i32, i32, vp, i32, i64, vp, vp, vp],
     "b2u_dice_ce_work_doubles": [i32, i32, i64, i32],
     "b2u_dice_ce_stats": [vp, vp, i32, i32, i32, vp, vp, vp, i32, i32, i64, vp],
     "b2u_dice_ce_finalize": [vp, vp, vp, vp, i32, i32, i64, i32, f32, f32, i32, i32, f32, vp],

@@ -276,6 +276,17 @@ int b2u_eval_edt(const uint8_t* border, int32_t Z, int32_t Y, int32_t X, double 
                  int32_t* scratch, double* dt, b2u_stream_t stream);
 int b2u_eval_sum_f64(const double* x, int64_t n, double* work, b2u_stream_t stream);
 
+/* ---- Keep-the-largest-component postprocessing (postprocessing/remove_connected_components.py:22-34
+ * `remove_all_but_largest_component_from_segmentation`, acvl-utils' `remove_all_but_largest_component`).
+ * b2u_pp_largest_component: mask = any(seg == labels[j]) with evaluation's comparison rule (labels: DEVICE int64
+ *   [n_labels], ascending and distinct, n_labels >= 0); its components with full connectivity (26 neighbours on the
+ *   C-contiguous [Z, Y, X] volume, Z*Y*X < 2^31; a lower-rank mask padded with leading unit axes); out = seg with every
+ *   masked voxel whose component is smaller than the largest set to `background` (the stored element's bits in the
+ *   low 1, 2 or 4 bytes).  Every component of the largest size is kept; an empty mask leaves out == seg.  dtype:
+ *   B2U_EVAL_* code.  work: int32 [2 * Z*Y*X + 1] (the component forest, the sizes, the largest size). */
+int b2u_pp_largest_component(const void* seg, int32_t dtype, int32_t Z, int32_t Y, int32_t X, const int64_t* labels,
+                             int32_t n_labels, int64_t background, void* out, int32_t* work, b2u_stream_t stream);
+
 /* ---- Dice + cross-entropy loss and online-validation statistics on the logits of the forward path
  * (training/loss/compound_losses.py:31-56 `DC_and_CE_loss`, dice.py:72-119 `MemoryEfficientSoftDiceLoss`,
  * robust_ce_loss.py:12-16, built at nnUNetTrainer.py:363-365; consumer nnUNetTrainer.py:961-1005 `validation_step`).
