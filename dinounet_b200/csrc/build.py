@@ -4,7 +4,7 @@ import subprocess
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-SOURCES = ["gemm_api.cu", ("gemm_tc2.cu", "gemm_tc2_bf16.o", ["-DB2U_GEMM2_TYPE=1"]), ("gemm_tc2.cu", "gemm_tc2_f16.o", ["-DB2U_GEMM2_TYPE=0"]), "attention_tc.cu", "attention_tc3.cu", "elementwise.cu", "fp32_tier.cu", "gemm_tf32.cu", "train_bwd.cu", "train_mode.cu", "msda.cu", "sliding_window.cu", "export.cu", "preprocess.cu", "evaluation.cu", "postprocessing.cu", "loss.cu", "host_util.cu"]
+SOURCES = ["gemm_api.cu", ("gemm_tc2.cu", "gemm_tc2_bf16.o", ["-DB2U_GEMM2_TYPE=1"]), ("gemm_tc2.cu", "gemm_tc2_f16.o", ["-DB2U_GEMM2_TYPE=0"]), "attention_tc.cu", "attention_tc3.cu", "elementwise.cu", "fp32_tier.cu", "gemm_tf32.cu", "train_bwd.cu", "train_mode.cu", "msda.cu", "sliding_window.cu", "export.cu", "preprocess.cu", "evaluation.cu", "postprocessing.cu", "augmentation.cu", "loss.cu", "host_util.cu"]
 # A/B builds: B2U_EXTRA_FLAGS="-DFOO=1" B2U_OUT_SUFFIX=_foo python build.py -> libdinounet_b200_foo.so (objects under build_foo/);
 # run with DINOUNET_B200_LIB=<that file>.  The default build takes neither.
 SUFFIX = os.environ.get("B2U_OUT_SUFFIX", "")

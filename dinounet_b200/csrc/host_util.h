@@ -21,6 +21,12 @@ int get_option(int key);
 // numpy's pairwise sum of a contiguous float64 x[n] (preprocess.cu's tree, shared with the float32 ZScore statistics):
 // the sum lands in work[0].  work: ceil(n / 8) doubles.
 int pairwise_sum_f64(const double* x, long long n, double* work, cudaStream_t stream);
+// numpy's float32 pairwise sum of each of `planes` contiguous runs of n (run p at x + p * n) into work[p * ws]; sq: of
+// (x - mean[p])^2.  work: planes * ws floats, ws >= ceil(n / 8).
+int pairwise_sum_planes_f32(const float* x, long long n, int planes, int sq, const float* mean, float* work,
+                            long long ws, cudaStream_t stream);
+// Exact min / max of each of `planes` contiguous runs of n into lo[p], hi[p].
+int minmax_planes_f32(const float* x, long long n, int planes, float* lo, float* hi, cudaStream_t stream);
 
 // Programmatic dependent launch (PDL), OPT-IN (option 5 = 1): every kernel of the forward plan can be launched with
 // cudaLaunchAttributeProgrammaticStreamSerialization; each calls `griddepcontrol.wait` before it touches global memory

@@ -37,10 +37,10 @@
 #include "common.cuh"
 #include "gemm_common.h"
 #include "host_util.h"
+#include "spline.cuh"
 
 namespace b2u {
 
-constexpr int kPad = 12;           // scipy's _prepad_for_spline_filter for mode 'nearest'
 constexpr int kLeaf = 128;         // numpy's PW_BLOCKSIZE
 constexpr long long kMinMaxChunk = 1 << 16;
 
@@ -117,9 +117,14 @@ __device__ __forceinline__ long long split_of(long long m) {
 
 // One thread per node of depth k (path bits, root decision first).  A leaf (m <= 128) writes its sum to val[o / 8]; an
 // inner node adds its children, both already evaluated at depth k + 1, into the slot it shares with its left child.
+// blockIdx.y is the plane of a batch of equal runs: x, stats and val advance by xs, ss and vs per plane.
 template <typename T>
 __global__ void __launch_bounds__(256) tree_level_kernel(const T* __restrict__ x, long long n, int k, Order3 ord,
-                                                         int sq, const T* __restrict__ stats, T* __restrict__ val) {
+                                                         int sq, const T* __restrict__ stats, T* __restrict__ val,
+                                                         long long xs, long long ss, long long vs) {
+  x += blockIdx.y * xs;
+  stats += blockIdx.y * ss;
+  val += blockIdx.y * vs;
   const long long b = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (b >= (1LL << k)) return;
   long long o = 0, m = n;
@@ -216,10 +221,6 @@ __global__ void __launch_bounds__(256) pad_kernel(const float* __restrict__ x, i
   }
 }
 
-struct FilterConsts {
-  double z, zn, gain, f_causal, f_anti;  // pole, z^n, (1-z)(1-1/z), z / (1 - z^n z^n), z / (z - 1)
-};
-
 // One thread per line of the contiguous [d0, d1, d2] array along `axis` (scipy's NI_SplineFilter1D, mode 'nearest').
 __global__ void __launch_bounds__(128) spline_filter_kernel(double* __restrict__ c, int d0, int d1, int d2, int axis,
                                                             FilterConsts k) {
@@ -236,46 +237,7 @@ __global__ void __launch_bounds__(128) spline_filter_kernel(double* __restrict__
   } else {
     base = l * d2; st = 1; n = d2;
   }
-  double* p = c + base;
-  for (int i = 0; i < n; ++i) p[i * st] = __dmul_rn(p[i * st], k.gain);
-  const double c0 = p[0];
-  double s = __dadd_rn(c0, __dmul_rn(k.zn, p[(n - 1) * st]));
-  double zi = k.z;
-  for (int i = 1; i < n; ++i) {
-    s = __dadd_rn(s, __dmul_rn(zi, __dadd_rn(p[i * st], __dmul_rn(k.zn, p[(n - 1 - i) * st]))));
-    zi = __dmul_rn(zi, k.z);
-  }
-  p[0] = __dadd_rn(__dmul_rn(s, k.f_causal), c0);
-  double prev = p[0];
-  for (int i = 1; i < n; ++i) {
-    prev = __dadd_rn(p[i * st], __dmul_rn(k.z, prev));
-    p[i * st] = prev;
-  }
-  double next = __dmul_rn(p[(n - 1) * st], k.f_anti);
-  p[(n - 1) * st] = next;
-  for (int i = n - 2; i >= 0; --i) {
-    next = __dmul_rn(k.z, __dsub_rn(next, p[i * st]));
-    p[i * st] = next;
-  }
-}
-
-struct Taps3 {
-  int start;  // first tap, as an index into the padded axis
-  double w[4];
-};
-
-__device__ __forceinline__ Taps3 cubic_taps(int k, double zoom) {
-  const double cc = __dadd_rn(__dsub_rn(__dmul_rn(__dadd_rn(static_cast<double>(k), 0.5), zoom), 0.5),
-                              static_cast<double>(kPad));
-  const double fl = floor(cc);
-  const double y = __dsub_rn(cc, fl), z = __dsub_rn(1.0, y);
-  Taps3 t;
-  t.start = static_cast<int>(fl) - 1;
-  t.w[0] = __ddiv_rn(__dmul_rn(__dmul_rn(z, z), z), 6.0);
-  t.w[1] = __ddiv_rn(__dadd_rn(__dmul_rn(__dmul_rn(__dmul_rn(y, y), __dsub_rn(y, 2.0)), 3.0), 4.0), 6.0);
-  t.w[2] = __ddiv_rn(__dadd_rn(__dmul_rn(__dmul_rn(__dmul_rn(z, z), __dsub_rn(z, 2.0)), 3.0), 4.0), 6.0);
-  t.w[3] = __dsub_rn(__dsub_rn(__dsub_rn(1.0, t.w[0]), t.w[1]), t.w[2]);
-  return t;
+  spline_filter_line<false>(c + base, st, n, k);
 }
 
 // One output row (z, Y) per blockIdx.y / blockIdx.z, columns over blockIdx.x * blockDim.x.  three_d = 0: coef is
@@ -301,13 +263,7 @@ __global__ void __launch_bounds__(128) zoom3_kernel(const double* __restrict__ c
       }
     }
   } else {
-    const double* pz = coef + zo * plane;
-#pragma unroll
-    for (int b = 0; b < 4; ++b) {
-      const double* row = pz + (ty.start + b) * Wp + tx.start;
-#pragma unroll
-      for (int c = 0; c < 4; ++c) t = __dadd_rn(t, __dmul_rn(__dmul_rn(row[c], ty.w[b]), tx.w[c]));
-    }
+    t = cubic16(coef + zo * plane, Wp, ty, tx);
   }
   const int g = kThreeD ? 0 : zo;
   t = fmin(fmax(t, lo[g]), hi[g]);  // np.clip(out, min, max): minimum(maximum(x, min), max)
@@ -352,15 +308,19 @@ static int tree_depth(long long n) {
 }
 
 // Evaluates the whole tree over x[n] (in the order `ord`; sq: sum of (x - stats[0])^2), deepest level first: the sum
-// lands in work[0].  work: ceil(n / 8) elements.
+// lands in work[0].  work: ceil(n / 8) elements.  A batch of `planes` equal runs: plane p reads x + p * xs, its mean at
+// stats + p * ss, and sums into work + p * ws.
 template <typename T>
 static int pairwise_sum_tree(const T* x, long long n, const Order3& ord, int sq, const T* stats, T* work,
-                             cudaStream_t stream, const char* what) {
+                             cudaStream_t stream, const char* what, int planes = 1, long long xs = 0,
+                             long long ss = 0, long long ws = 0) {
   const int depth = tree_depth(n);
   if (depth > 40) return set_error(-1, "%s: tree depth %d", what, depth);
+  if (planes < 1 || planes > 65535) return set_error(-1, "%s: %d planes", what, planes);
   for (int k = depth; k >= 0; --k) {
     const long long nodes = 1LL << k;
-    tree_level_kernel<T><<<static_cast<unsigned>((nodes + 255) / 256), 256, 0, stream>>>(x, n, k, ord, sq, stats, work);
+    const dim3 grid(static_cast<unsigned>((nodes + 255) / 256), planes);
+    tree_level_kernel<T><<<grid, 256, 0, stream>>>(x, n, k, ord, sq, stats, work, xs, ss, ws);
     int rc = check_launch(what);
     if (rc) return rc;
   }
@@ -369,6 +329,17 @@ static int pairwise_sum_tree(const T* x, long long n, const Order3& ord, int sq,
 
 int pairwise_sum_f64(const double* x, long long n, double* work, cudaStream_t stream) {
   return pairwise_sum_tree<double>(x, n, Order3{1, n, 0, 0, 1, true}, 0, nullptr, work, stream, "pairwise_sum_f64");
+}
+
+int pairwise_sum_planes_f32(const float* x, long long n, int planes, int sq, const float* mean, float* work,
+                            long long ws, cudaStream_t stream) {
+  return pairwise_sum_tree<float>(x, n, Order3{1, n, 0, 0, 1, true}, sq, mean, work, stream, "pairwise_sum_planes_f32",
+                                  planes, n, 1, ws);
+}
+
+int minmax_planes_f32(const float* x, long long n, int planes, float* lo, float* hi, cudaStream_t stream) {
+  minmax_kernel<float><<<planes, 256, 0, stream>>>(x, x, n * planes, n, lo, hi, nullptr);
+  return check_launch("minmax_planes_f32");
 }
 
 }  // namespace b2u

@@ -106,6 +106,9 @@ SIGNATURES = {
     "b2u_eval_edt": [vp, i32, i32, i32, C.c_double, C.c_double, C.c_double, vp, vp, vp, vp],
     "b2u_eval_sum_f64": [vp, i64, vp, vp],
     "b2u_pp_largest_component": [vp, i32, i32, i32, i32, vp, i32, i64, vp, vp, vp],
+    "b2u_aug_work_bytes": [i32, i32, i32, i32, i32, i32],
+    "b2u_aug_apply": [vp, vp, i32, i32, i32, i32, i32, i32, vp, vp, C.c_uint64, vp, i32, vp, vp, vp, vp],
+    "b2u_aug_noise_field": [C.c_uint64, i32, i32, i64, vp, vp],
     "b2u_dice_ce_work_doubles": [i32, i32, i64, i32],
     "b2u_dice_ce_stats": [vp, vp, i32, i32, i32, vp, vp, vp, i32, i32, i64, vp],
     "b2u_dice_ce_finalize": [vp, vp, vp, vp, i32, i32, i64, i32, f32, f32, i32, i32, f32, vp],
@@ -171,7 +174,8 @@ SIGNATURES = {
 }
 _RESTYPES = {"b2u_last_error": C.c_char_p, "b2u_launch_count": C.c_int64, "b2u_in_stats_work_floats": C.c_int64,
              "b2u_dice_ce_work_doubles": C.c_int64, "b2u_dice_bce_work_doubles": C.c_int64,
-             "b2u_f32_bn_work_doubles": C.c_int64, "b2u_pre_resample3_work_doubles": C.c_int64}
+             "b2u_f32_bn_work_doubles": C.c_int64, "b2u_pre_resample3_work_doubles": C.c_int64,
+             "b2u_aug_work_bytes": C.c_int64}
 
 _lib: Optional[C.CDLL] = None
 

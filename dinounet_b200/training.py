@@ -8,6 +8,7 @@ works unchanged; otherwise they derive from `object` (the hook itself is a stati
 """
 from typing import List, Tuple, Union
 
+import numpy as np
 import torch
 from torch import nn
 
@@ -26,14 +27,17 @@ class DinoUNetTrainer(_Base):
     _dinov3_pretrained_path = None
     _dinov3_model_name = None
     _train_semantics = None
+    _device_augmentation = False
 
     @classmethod
     def set_network_config(cls, network_config, dinov3_pretrained_path=None, dinov3_model_name=None,
-                           adapter_type="default", train_semantics=None):
+                           adapter_type="default", train_semantics=None, device_augmentation=False):
         """train_semantics: `DinoUNet.train_semantics` of the networks `build_network_architecture` returns ("oracle" or
-        "reference"); None keeps the module default."""
+        "reference"); None keeps the module default.  device_augmentation: run the training transforms on the device
+        (dinounet_b200/augmentation.py) instead of batchgenerators' worker processes; off by default."""
         cls._network_config = network_config
         cls._train_semantics = train_semantics
+        cls._device_augmentation = bool(device_augmentation)
         if dinov3_pretrained_path is not None:
             cls._dinov3_pretrained_path = dinov3_pretrained_path
         if dinov3_model_name is not None:
@@ -43,6 +47,7 @@ class DinoUNetTrainer(_Base):
         DinoUNetTrainer._dinov3_model_name = cls._dinov3_model_name
         DinoUNetTrainer._dinov3_pretrained_path = cls._dinov3_pretrained_path
         DinoUNetTrainer._train_semantics = cls._train_semantics
+        DinoUNetTrainer._device_augmentation = cls._device_augmentation
 
     @staticmethod
     def build_network_architecture(architecture_class_name: str, arch_init_kwargs: dict,
@@ -62,6 +67,40 @@ class DinoUNetTrainer(_Base):
             net.train_semantics = DinoUNetTrainer._train_semantics
         return net
 
+
+    # ---- training transforms (nnUNetTrainer.py:684-775)
+    @staticmethod
+    def get_training_transforms(patch_size, rotation_for_DA, deep_supervision_scales, mirror_axes,
+                                do_dummy_2d_data_aug, *args, **kwargs):
+        """With device augmentation on, the host pipeline only renames `seg` to `target` and makes tensors of the
+        batch at the initial patch size (float32 data, int16 seg); `train_step` augments it on the device.  Otherwise
+        the reference's pipeline."""
+        if DinoUNetTrainer._device_augmentation:
+            return PassThroughTransforms()
+        return _Base.get_training_transforms(patch_size, rotation_for_DA, deep_supervision_scales, mirror_axes,
+                                             do_dummy_2d_data_aug, *args, **kwargs)
+
+    def _device_augmenter(self):
+        """The device pipeline with the trainer's configuration, built once.  Under DDP each rank seeds its own stream
+        of draws: the seed is derived from the rank."""
+        aug = getattr(self, "_device_aug", None)
+        if aug is None:
+            from .augmentation import DeviceTrainingAugmentation
+            rotation_for_DA, do_dummy_2d, _, mirror_axes = self.configure_rotation_dummyDA_mirroring_and_inital_patch_size()
+            if do_dummy_2d or len(self.configuration_manager.patch_size) != 2:
+                raise NotImplementedError("device augmentation covers 2-D configurations only")
+            lm = self.label_manager
+            rank = getattr(self, "local_rank", 0) if getattr(self, "is_ddp", False) else 0
+            seed = int(np.random.SeedSequence(self._device_augmentation_seed, spawn_key=(rank,)).generate_state(1)[0])
+            aug = DeviceTrainingAugmentation(self.configuration_manager.patch_size, rotation_for_DA, mirror_axes,
+                                             use_mask_for_norm=self.configuration_manager.use_mask_for_norm,
+                                             regions=lm.foreground_regions if lm.has_regions else None,
+                                             ignore_label=lm.ignore_label, seed=seed)
+            self._device_aug = aug
+        return aug
+
+    # None: fresh entropy per run; an int makes every rank's draws reproducible
+    _device_augmentation_seed = None
 
     # ---- forward-only callers of the path that the trainer owns (nnUNetTrainer.py:355-365, :945-1005)
     def _build_loss(self):
@@ -97,6 +136,8 @@ class DinoUNetTrainer(_Base):
         if isinstance(target, list):
             target = target[0]
         target = target.to(self.device, non_blocking=True)
+        if DinoUNetTrainer._device_augmentation:
+            data, target = self._device_augmenter()(data, target)
         net = self.network.module if hasattr(self.network, "module") else self.network
         loss = train_step(net, self.loss, self.optimizer, data, target)
         return {"loss": loss.cpu().numpy()}
@@ -113,6 +154,16 @@ class DinoUNetTrainer(_Base):
             output = self.network(data)
         del data
         return validation_statistics(self.loss, output, target)
+
+
+class PassThroughTransforms:
+    """The host side of device augmentation: `seg` renamed to `target`, data and seg as tensors (NumpyToTensor without
+    the cast of the labels to float, so that they stay int16 for the device pipeline)."""
+
+    def __call__(self, **data_dict):
+        data_dict["data"] = torch.as_tensor(np.asarray(data_dict["data"], dtype=np.float32))
+        data_dict["target"] = torch.as_tensor(np.asarray(data_dict.pop("seg"), dtype=np.int16))
+        return data_dict
 
 
 class DinoUNetTrainer_s(DinoUNetTrainer):

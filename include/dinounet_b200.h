@@ -287,6 +287,24 @@ int b2u_eval_sum_f64(const double* x, int64_t n, double* work, b2u_stream_t stre
 int b2u_pp_largest_component(const void* seg, int32_t dtype, int32_t Z, int32_t Y, int32_t X, const int64_t* labels,
                              int32_t n_labels, int64_t background, void* out, int32_t* work, b2u_stream_t stream);
 
+/* ---- Training augmentation of 2-D batches (nnUNetTrainer.get_training_transforms, nnUNetTrainer.py:684-775, as
+ * batchgenerators 0.25 runs it; dinounet_b200/augmentation.py writes the record and restates the draws).
+ * b2u_aug_apply: data fp32 [B, C, h, w] and seg int16 [B, 1, h, w] at the initial patch size -> out fp32 [B, C, H, W]
+ *   and target fp32 ([B, 1, H, W] label map, or [B, R, H, W] regions), h >= H, w >= W, B*C <= 65535.  rec: DEVICE
+ *   double [B*C, B2U_AUG_REC], every decision of every transform (field layout in csrc/augmentation.cu).  consts: HOST
+ *   double[5] {pole, pole^(h-1), pole^(w-1), gain, pole^2 - 1} of the spatial transform's spline prefilter (mirror
+ *   boundaries).  seed keys the Gaussian noise (b2u_aug_noise_field).  regions: DEVICE int32 [R + 1 offsets, labels],
+ *   region q is labels[offsets[q] .. offsets[q+1]); R = 0 writes the label map.  work: b2u_aug_work_bytes bytes.  No
+ *   host synchronisation; the launch sequence does not depend on the record.
+ * b2u_aug_noise_field: the standard-normal field the noise step adds (times its std), fp64 [B, C, n]: Philox4x32-10
+ *   keyed by seed, counter (pixel / 2, channel, sample), Box-Muller on two 53-bit uniforms. */
+#define B2U_AUG_REC 40
+int64_t b2u_aug_work_bytes(int32_t B, int32_t C, int32_t h, int32_t w, int32_t H, int32_t W);
+int b2u_aug_apply(const float* data, const int16_t* seg, int32_t B, int32_t C, int32_t h, int32_t w, int32_t H,
+                  int32_t W, const double* rec, const double* consts, uint64_t seed, const int32_t* regions, int32_t R,
+                  void* work, float* out, float* target, b2u_stream_t stream);
+int b2u_aug_noise_field(uint64_t seed, int32_t B, int32_t C, int64_t n, double* out, b2u_stream_t stream);
+
 /* ---- Dice + cross-entropy loss and online-validation statistics on the logits of the forward path
  * (training/loss/compound_losses.py:31-56 `DC_and_CE_loss`, dice.py:72-119 `MemoryEfficientSoftDiceLoss`,
  * robust_ce_loss.py:12-16, built at nnUNetTrainer.py:363-365; consumer nnUNetTrainer.py:961-1005 `validation_step`).
