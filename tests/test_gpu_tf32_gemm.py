@@ -3,7 +3,8 @@ of its parameter block, against fp64 torch references computed on TF32-ROUNDED o
 mantissa bits = cvt.rna.tf32.f32, emulated bit-exactly below): what remains is fp32 accumulation order, so the
 tolerance is 2e-4 of the largest output (a misplaced chunk / swizzle / descriptor is an O(1) error).  Then the three
 autograd Functions that use it (Linear, Conv3x3, ConvT2x2: forward, data gradient, weight gradient, bias gradient)
-against fp64 autograd on the UNROUNDED operands at TF32's own precision (3e-3).
+against fp64 autograd on the UNROUNDED operands at TF32's own precision (3e-3), and the same Functions on the fp32 SIMT
+tier (`b2u_f32_gemm`) at 2e-5.
 
 The reference formulas of this file are themselves checked WITHOUT a GPU by tests/test_tf32_gemm_refs_cpu.py, which runs
 the same test bodies against a slow torch emulation of the parameter block's addressing (`DEV`, `raw_gemm` are the seams)."""
@@ -192,12 +193,27 @@ def test_tensor_core_tier_matches_the_fp32_tier_and_counts_as_native():
 
 
 def test_autograd_functions_against_fp64_autograd():
-    """LinearF / Conv3x3F / ConvT2x2F forward + backward on the tensor-core tier vs torch fp64 autograd (unrounded operands)."""
+    """LinearF / Conv3x3F / ConvT2x2F forward + backward on the tensor-core tier vs torch fp64 autograd (unrounded operands)
+    at TF32's own precision."""
+    _autograd_functions_against_fp64_autograd("tf32", 3e-3)
+
+
+def test_fp32_tier_autograd_functions_against_fp64_autograd():
+    """The same Functions and shapes on the fp32 SIMT tier (b2u_f32_gemm, the gradient goldens' tier) at fp32 accumulation's
+    precision (2e-5, an estimate)."""
+    _autograd_functions_against_fp64_autograd("fp32", 2e-5)
+
+
+def _autograd_functions_against_fp64_autograd(tier, tol):
+    """The stride-2 convolutions include the SPM's shapes at 512^2, whose data gradient is b2u_f32_conv3x3_dgrad on both
+    tiers; the last transposed conv is the decoder's at 512^2, whose bias gradient sums 524288 rows (f32_colsum's 64-split
+    branch)."""
     from dinounet_b200 import train_path as TP
-    prev, TP._GEMM_TIER = TP._GEMM_TIER, "tf32"
+    prev, TP._GEMM_TIER = TP._GEMM_TIER, tier
     try:
         def cmp(got, want, what):
-            check(got.detach(), want.detach().double(), tol=3e-3, what=what)
+            err = check(got.detach(), want.detach().double(), tol=tol, what=f"{tier} {what}")
+            print(f"{tier} {what}: rel err {err:.2e}")
 
         M, K, N = 5000, 192, 96                                       # Linear with bias and residual
         x, W, b, r = [t.requires_grad_() for t in (rnd(M, K, seed=1), rnd(N, K, seed=2, scale=0.1), rnd(N, seed=3), rnd(M, N, seed=4))]
@@ -209,8 +225,10 @@ def test_autograd_functions_against_fp64_autograd():
         yd.backward(g.double())
         for got, want, what in ((y, yd, "y"), (x.grad, xd.grad, "dx"), (W.grad, Wd_.grad, "dW"), (b.grad, bd.grad, "db"), (r.grad, rd.grad, "dres")):
             cmp(got, want, "linear " + what)
-        for stride in (1, 2):                                         # Conv3x3
-            B, H, Wd, Cin, Cout = 2, 32, 32, 64, 32
+        # Conv3x3: (B, H, Cin, Cout, stride); the stride-2 rows after the first two are the SPM's conv2..conv4 at 512^2
+        for B, H, Cin, Cout, stride in ((2, 32, 64, 32, 1), (2, 32, 64, 32, 2), (2, 128, 64, 128, 2), (2, 64, 128, 256, 2),
+                                        (2, 32, 256, 256, 2), (1, 24, 20, 7, 2)):
+            Wd = H
             x, Wt, b = [t.requires_grad_() for t in (rnd(B * H * Wd, Cin, seed=6), rnd(Cout, Cin, 3, 3, seed=7, scale=0.1), rnd(Cout, seed=8))]
             y = TP.Conv3x3F.apply(x, Wt, b, B, H, Wd, stride)
             g = rnd(*y.shape, seed=9)
@@ -219,16 +237,16 @@ def test_autograd_functions_against_fp64_autograd():
             yd = F.conv2d(xd.view(B, H, Wd, Cin).permute(0, 3, 1, 2), Wtd, bd, stride=stride, padding=1).permute(0, 2, 3, 1).reshape(y.shape)
             yd.backward(g.double())
             for got, want, what in ((y, yd, "y"), (x.grad, xd.grad, "dx"), (Wt.grad, Wtd.grad, "dW"), (b.grad, bd.grad, "db")):
-                cmp(got, want, f"conv s{stride} " + what)
-        B, h, w, Cin, Cout = 2, 16, 16, 64, 32                        # ConvTranspose 2x2
-        x, Wt, b = [t.requires_grad_() for t in (rnd(B * h * w, Cin, seed=10), rnd(Cin, Cout, 2, 2, seed=11, scale=0.1), rnd(Cout, seed=12))]
-        y = TP.ConvT2x2F.apply(x, Wt, b, B, h, w)
-        g = rnd(*y.shape, seed=13)
-        y.backward(g)
-        xd, Wtd, bd = [t.detach().double().requires_grad_() for t in (x, Wt, b)]
-        yd = F.conv_transpose2d(xd.view(B, h, w, Cin).permute(0, 3, 1, 2), Wtd, bd, stride=2).permute(0, 2, 3, 1).reshape(y.shape)
-        yd.backward(g.double())
-        for got, want, what in ((y, yd, "y"), (x.grad, xd.grad, "dx"), (Wt.grad, Wtd.grad, "dW"), (b.grad, bd.grad, "db")):
-            cmp(got, want, "convT " + what)
+                cmp(got, want, f"conv s{stride} {B}x{H}x{H}x{Cin}->{Cout} " + what)
+        for B, h, w, Cin, Cout in ((2, 16, 16, 64, 32), (2, 256, 256, 64, 32)):          # ConvTranspose 2x2
+            x, Wt, b = [t.requires_grad_() for t in (rnd(B * h * w, Cin, seed=10), rnd(Cin, Cout, 2, 2, seed=11, scale=0.1), rnd(Cout, seed=12))]
+            y = TP.ConvT2x2F.apply(x, Wt, b, B, h, w)
+            g = rnd(*y.shape, seed=13)
+            y.backward(g)
+            xd, Wtd, bd = [t.detach().double().requires_grad_() for t in (x, Wt, b)]
+            yd = F.conv_transpose2d(xd.view(B, h, w, Cin).permute(0, 3, 1, 2), Wtd, bd, stride=2).permute(0, 2, 3, 1).reshape(y.shape)
+            yd.backward(g.double())
+            for got, want, what in ((y, yd, "y"), (x.grad, xd.grad, "dx"), (Wt.grad, Wtd.grad, "dW"), (b.grad, bd.grad, "db")):
+                cmp(got, want, f"convT {B}x{h}x{w}x{Cin}->{Cout} " + what)
     finally:
         TP._GEMM_TIER = prev
