@@ -21,6 +21,8 @@ int get_option(int key);
 // numpy's pairwise sum of a contiguous float64 x[n] (preprocess.cu's tree, shared with the float32 ZScore statistics):
 // the sum lands in work[0].  work: ceil(n / 8) doubles.
 int pairwise_sum_f64(const double* x, long long n, double* work, cudaStream_t stream);
+// The same float64 sum of (x - mean[0])^2, numpy's `_var` pass.
+int pairwise_sum_sq_f64(const double* x, long long n, const double* mean, double* work, cudaStream_t stream);
 // numpy's float32 pairwise sum of each of `planes` contiguous runs of n (run p at x + p * n) into work[p * ws]; sq: of
 // (x - mean[p])^2.  work: planes * ws floats, ws >= ceil(n / 8).
 int pairwise_sum_planes_f32(const float* x, long long n, int planes, int sq, const float* mean, float* work,

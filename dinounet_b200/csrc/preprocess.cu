@@ -331,6 +331,10 @@ int pairwise_sum_f64(const double* x, long long n, double* work, cudaStream_t st
   return pairwise_sum_tree<double>(x, n, Order3{1, n, 0, 0, 1, true}, 0, nullptr, work, stream, "pairwise_sum_f64");
 }
 
+int pairwise_sum_sq_f64(const double* x, long long n, const double* mean, double* work, cudaStream_t stream) {
+  return pairwise_sum_tree<double>(x, n, Order3{1, n, 0, 0, 1, true}, 1, mean, work, stream, "pairwise_sum_sq_f64");
+}
+
 int pairwise_sum_planes_f32(const float* x, long long n, int planes, int sq, const float* mean, float* work,
                             long long ws, cudaStream_t stream) {
   return pairwise_sum_tree<float>(x, n, Order3{1, n, 0, 0, 1, true}, sq, mean, work, stream, "pairwise_sum_planes_f32",

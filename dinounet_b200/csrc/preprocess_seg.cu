@@ -18,6 +18,8 @@
 //   b2u_pre_seg_compact   np.argwhere order of one class: the ascending linear indices of its voxels (block counts, one
 //                         scan, an in-order scatter).
 //   b2u_pre_seg_gather    rows[i] = (0, z, y, x) of the voxel of rank ranks[i] in that list (the host draws the ranks).
+//   b2u_fp_fg_compact     the same compaction for the fingerprint's foreground `seg > 0` (fingerprint_extractor.py:60),
+//                         and its voxel count.
 #include <algorithm>
 #include <climits>
 
@@ -168,15 +170,31 @@ __global__ void __launch_bounds__(kSegThreads) seg_count_kernel(const void* __re
     if (block_counts[k]) atomicAdd(counts + k, static_cast<unsigned long long>(block_counts[k]));
 }
 
-// block_counts[b] = the class's voxels in [b * kCompactChunk, (b + 1) * kCompactChunk).
+// The compaction's predicates: membership in a sorted label set, or numpy's `seg > 0` (a NaN voxel is not foreground).
+struct InLabels {
+  const long long* labels;
+  int n;
+  __device__ __forceinline__ bool operator()(const void* seg, int dtype, long long i) const {
+    return in_sorted_labels(seg, dtype, i, labels, n);
+  }
+};
+
+struct Positive {
+  __device__ __forceinline__ bool operator()(const void* seg, int dtype, long long i) const {
+    if (dtype == B2U_EVAL_F32) return static_cast<const float*>(seg)[i] > 0.f;
+    return load_int_label(seg, dtype, i) > 0;
+  }
+};
+
+// block_counts[b] = the voxels in [b * kCompactChunk, (b + 1) * kCompactChunk) that satisfy `pred`.
+template <typename Pred>
 __global__ void __launch_bounds__(kSegThreads) compact_count_kernel(const void* __restrict__ seg, int dtype, long long n,
-                                                                    const long long* __restrict__ labels, int n_labels,
-                                                                    int32_t* __restrict__ block_counts) {
+                                                                    Pred pred, int32_t* __restrict__ block_counts) {
   const long long b = static_cast<long long>(blockIdx.x) * kCompactChunk, e = min(n, b + kCompactChunk);
   int c = 0;
   for (long long t = b; t < e; t += kCompactTile) {
     const long long i = t + threadIdx.x;
-    c += __syncthreads_count(i < e && in_sorted_labels(seg, dtype, i, labels, n_labels));
+    c += __syncthreads_count(i < e && pred(seg, dtype, i));
   }
   if (threadIdx.x == 0) block_counts[blockIdx.x] = c;
 }
@@ -216,32 +234,35 @@ __global__ void __launch_bounds__(1024) exclusive_scan_kernel(int32_t* __restric
   }
 }
 
-// Block b writes the linear indices of its chunk's class voxels, ascending, at idx[offsets[b] ...].
+// Block b writes the linear indices of its chunk's voxels that satisfy `pred`, ascending, at idx[offsets[b] ...]; the
+// last block stores the total in *total when it is not null.
+template <typename Pred>
 __global__ void __launch_bounds__(kSegThreads) compact_scatter_kernel(const void* __restrict__ seg, int dtype,
-                                                                      long long n, const long long* __restrict__ labels,
-                                                                      int n_labels,
+                                                                      long long n, Pred pred,
                                                                       const int32_t* __restrict__ offsets,
-                                                                      int32_t* __restrict__ idx) {
+                                                                      int32_t* __restrict__ idx,
+                                                                      int64_t* __restrict__ total) {
   __shared__ int warp_sums[kSegThreads / 32];
   const long long b = static_cast<long long>(blockIdx.x) * kCompactChunk, e = min(n, b + kCompactChunk);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   int base = offsets[blockIdx.x];
   for (long long t = b; t < e; t += kCompactTile) {
     const long long i = t + threadIdx.x;
-    const bool hit = i < e && in_sorted_labels(seg, dtype, i, labels, n_labels);
+    const bool hit = i < e && pred(seg, dtype, i);
     const unsigned ballot = __ballot_sync(0xffffffffu, hit);
     if (lane == 0) warp_sums[warp] = __popc(ballot);
     __syncthreads();
-    int before = 0, total = 0;
+    int before = 0, sum = 0;
 #pragma unroll
     for (int q = 0; q < kSegThreads / 32; ++q) {
       before += q < warp ? warp_sums[q] : 0;
-      total += warp_sums[q];
+      sum += warp_sums[q];
     }
     if (hit) idx[base + before + __popc(ballot & ((1u << lane) - 1u))] = static_cast<int32_t>(i);
-    base += total;
+    base += sum;
     __syncthreads();
   }
+  if (total && threadIdx.x == 0 && blockIdx.x == gridDim.x - 1) *total = base;
 }
 
 __global__ void __launch_bounds__(kSegThreads) gather_rows_kernel(const int32_t* __restrict__ idx,
@@ -272,6 +293,21 @@ static void launch_resample(const void* seg, int Z, int h, int w, int H, int W, 
   resample_seg_kernel<T><<<grid, 128, 0, stream>>>(static_cast<const T*>(seg), h, w, H, W,
                                                    static_cast<double>(h) / H, static_cast<double>(w) / W,
                                                    static_cast<T*>(out), out_max);
+}
+
+// count -> exclusive scan -> in-order scatter of the voxels that satisfy `pred`.
+template <typename Pred>
+static int compact(const void* seg, int dtype, long long n, Pred pred, int32_t* work, int32_t* idx, int64_t* total,
+                   cudaStream_t stream, const char* what) {
+  const long long blocks = (n + kCompactChunk - 1) / kCompactChunk;
+  compact_count_kernel<Pred><<<static_cast<unsigned>(blocks), kSegThreads, 0, stream>>>(seg, dtype, n, pred, work);
+  int rc = check_launch(what);
+  if (rc) return rc;
+  exclusive_scan_kernel<<<1, 1024, 0, stream>>>(work, static_cast<int>(blocks));
+  if ((rc = check_launch(what))) return rc;
+  compact_scatter_kernel<Pred><<<static_cast<unsigned>(blocks), kSegThreads, 0, stream>>>(seg, dtype, n, pred, work,
+                                                                                           idx, total);
+  return check_launch(what);
 }
 
 }  // namespace b2u
@@ -328,16 +364,17 @@ extern "C" int b2u_pre_seg_compact(const void* seg, int32_t dtype, int64_t n, co
   if (n <= 0 || n > INT_MAX || !valid_dtype(dtype) || n_labels < 1)
     return set_error(-1, "b2u_pre_seg_compact: n=%lld dtype=%d n_labels=%d", static_cast<long long>(n), dtype,
                      n_labels);
-  const long long blocks = b2u_pre_seg_compact_work_ints(n);
-  const long long* lab = reinterpret_cast<const long long*>(labels);
-  compact_count_kernel<<<static_cast<unsigned>(blocks), kSegThreads, 0, stream>>>(seg, dtype, n, lab, n_labels, work);
-  int rc = check_launch("pre_seg_compact_count");
-  if (rc) return rc;
-  exclusive_scan_kernel<<<1, 1024, 0, stream>>>(work, static_cast<int>(blocks));
-  if ((rc = check_launch("pre_seg_compact_scan"))) return rc;
-  compact_scatter_kernel<<<static_cast<unsigned>(blocks), kSegThreads, 0, stream>>>(seg, dtype, n, lab, n_labels, work,
-                                                                                     idx);
-  return check_launch("pre_seg_compact_scatter");
+  return compact(seg, dtype, n, InLabels{reinterpret_cast<const long long*>(labels), n_labels}, work, idx, nullptr,
+                 stream, "pre_seg_compact");
+}
+
+extern "C" int b2u_fp_fg_compact(const void* seg, int32_t dtype, int64_t n, int32_t* work, int32_t* idx, int64_t* count,
+                                 b2u_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (!seg || !work || !idx || !count) return set_error(-1, "b2u_fp_fg_compact: null pointer");
+  if (n <= 0 || n > INT_MAX || !valid_dtype(dtype))
+    return set_error(-1, "b2u_fp_fg_compact: n=%lld dtype=%d", static_cast<long long>(n), dtype);
+  return compact(seg, dtype, n, Positive{}, work, idx, count, stream, "fp_fg_compact");
 }
 
 extern "C" int b2u_pre_seg_gather(const int32_t* idx, const int64_t* ranks, int64_t t, int32_t H, int32_t W,

@@ -108,6 +108,12 @@ SIGNATURES = {
     "b2u_pre_seg_compact_work_ints": [i64],
     "b2u_pre_seg_compact": [vp, i32, i64, vp, i32, vp, vp, vp],
     "b2u_pre_seg_gather": [vp, vp, i64, i32, i32, vp, vp],
+    "b2u_fp_fg_compact": [vp, i32, i64, vp, vp, vp, vp],
+    "b2u_fp_gather": [vp, i32, i64, vp, vp, i64, vp, i64, vp],
+    "b2u_fp_select_work_bytes": [],
+    "b2u_fp_select": [vp, i64, vp, i32, vp, vp, vp],
+    "b2u_fp_moments_work_bytes": [i64, i32],
+    "b2u_fp_moments": [vp, i64, i32, i32, vp, vp, vp],
     "b2u_eval_masks": [vp, i32, vp, i32, i32, i32, i32, i32, C.POINTER(C.c_int64), i32, i32, i64, vp, vp, vp, vp],
     "b2u_eval_edt": [vp, i32, i32, i32, C.c_double, C.c_double, C.c_double, vp, vp, vp, vp],
     "b2u_eval_sum_f64": [vp, i64, vp, vp],
@@ -181,7 +187,8 @@ SIGNATURES = {
 _RESTYPES = {"b2u_last_error": C.c_char_p, "b2u_launch_count": C.c_int64, "b2u_in_stats_work_floats": C.c_int64,
              "b2u_dice_ce_work_doubles": C.c_int64, "b2u_dice_bce_work_doubles": C.c_int64,
              "b2u_f32_bn_work_doubles": C.c_int64, "b2u_pre_resample3_work_doubles": C.c_int64,
-             "b2u_aug_work_bytes": C.c_int64, "b2u_pre_seg_compact_work_ints": C.c_int64}
+             "b2u_aug_work_bytes": C.c_int64, "b2u_pre_seg_compact_work_ints": C.c_int64,
+             "b2u_fp_select_work_bytes": C.c_int64, "b2u_fp_moments_work_bytes": C.c_int64}
 
 _lib: Optional[C.CDLL] = None
 

@@ -23,8 +23,10 @@ reference's normalization mask `seg >= 0` is then all true, so the data are comp
 batchgenerators' `resize_segmentation(order=1)` in one pass (csrc/preprocess_seg.cu: `b2u_pre_resample_seg`) and
 returned as an int8 / int16 device tensor by the reference's `np.max(seg) > 127` rule, and
 `properties["class_locations"]` gets `_sample_foreground_locations`' keys and rows (`b2u_pre_seg_count`,
-`b2u_pre_seg_compact`, `b2u_pre_seg_gather`; the RandomState draws stay on the host).  Not implemented: the dataset
-loop `run` (a spawn pool over the cases), the `modify_seg_fn` hook, and the cascade's previous-stage segmentation.
+`b2u_pre_seg_compact`, `b2u_pre_seg_gather`; the RandomState draws stay on the host).  `run` is the dataset loop
+(default_preprocessor.py:197-260) without the spawn pool: the cases run in order on the current device while threads
+read the next cases and compress and write the finished ones.  Not implemented: the `modify_seg_fn` hook and the
+cascade's previous-stage segmentation.
 
 Input of another dtype is cast to float32 on the device first, as the reference's image readers deliver it (for such
 input the reference's `run_case_npy` would write the normalized values back into the input's dtype).  The case is
@@ -40,7 +42,10 @@ ZScore tree slots.
 import ctypes
 import json
 import math
+import os
 import pickle
+import shutil
+from concurrent.futures import ThreadPoolExecutor
 from typing import Sequence
 
 import numpy as np
@@ -295,9 +300,7 @@ class DevicePreprocessor:
         if isinstance(dataset_json, str):
             with open(dataset_json) as f:
                 dataset_json = json.load(f)
-        rw = plans_manager.image_reader_writer_class()
-        data, data_properties = rw.read_images(image_files)
-        seg = rw.read_seg(seg_file)[0] if seg_file is not None else None
+        data, seg, data_properties = _read_case(image_files, seg_file, plans_manager)
         data, seg = self.run_case_npy(data, seg, data_properties, plans_manager, configuration_manager, dataset_json)
         return data, seg, data_properties
 
@@ -306,9 +309,90 @@ class DevicePreprocessor:
         """DefaultPreprocessor.run_case_save (lines 148-154): `<name>.npz` (data, seg as host arrays, compressed) and the
         properties pickled to `<name>.pkl`, the files the trainer loads."""
         data, seg, properties = self.run_case(image_files, seg_file, plans_manager, configuration_manager, dataset_json)
-        np.savez_compressed(output_filename_truncated + ".npz", data=_host(data), seg=_host(seg))
-        with open(output_filename_truncated + ".pkl", "wb") as f:
-            pickle.dump(properties, f)
+        _save_case(output_filename_truncated, _host(data), _host(seg), properties)
+
+    def run(self, dataset_name_or_id, configuration_name: str, plans_identifier: str, num_processes: int):
+        """DefaultPreprocessor.run (default_preprocessor.py:197-260): the plans and dataset.json of the preprocessed
+        folder, a fresh `<data_identifier>/` and one `<case>.npz` / `<case>.pkl` per training case, each what
+        `run_case_save` writes.  The cases run in order on the current device; `num_processes` threads read the next
+        cases ahead and as many compress and write the finished ones."""
+        dataset_name = _dataset_name(dataset_name_or_id)
+        raw, preprocessed = _raw_and_preprocessed()
+        assert os.path.isdir(os.path.join(raw, dataset_name)), "The requested dataset could not be found in nnUNet_raw"
+        plans_file = os.path.join(preprocessed, dataset_name, plans_identifier + ".json")
+        assert os.path.isfile(plans_file), "Expected plans file (%s) not found. Run corresponding " \
+                                           "nnUNet_plan_experiment first." % plans_file
+        with open(plans_file) as f:
+            plans_manager = _plans_manager(json.load(f))
+        configuration_manager = plans_manager.get_configuration(configuration_name)
+        if self.verbose:
+            print(f"Preprocessing the following configuration: {configuration_name}")
+            print(configuration_manager)
+        with open(os.path.join(preprocessed, dataset_name, "dataset.json")) as f:
+            dataset_json = json.load(f)
+        output_directory = os.path.join(preprocessed, dataset_name, configuration_manager.data_identifier)
+        if os.path.isdir(output_directory):
+            shutil.rmtree(output_directory)
+        os.makedirs(output_directory, exist_ok=True)
+        dataset = _get_filenames_of_train_images_and_targets(os.path.join(raw, dataset_name), dataset_json)
+        keys = list(dataset.keys())
+        workers = max(1, int(num_processes))
+        with ThreadPoolExecutor(workers) as readers, ThreadPoolExecutor(workers) as writers:
+            reads = [readers.submit(_read_case, dataset[k]["images"], dataset[k]["label"], plans_manager)
+                     for k in keys[:workers]]
+            writes = []
+            for i, k in enumerate(keys):
+                data, seg, properties = reads[i].result()
+                if i + workers < len(keys):
+                    nk = keys[i + workers]
+                    reads.append(readers.submit(_read_case, dataset[nk]["images"], dataset[nk]["label"], plans_manager))
+                data, seg = self.run_case_npy(data, seg, properties, plans_manager, configuration_manager,
+                                              dataset_json)
+                writes.append(writers.submit(_save_case, os.path.join(output_directory, k), _host(data), _host(seg),
+                                             properties))
+                reads[i] = None
+                while len([w for w in writes if not w.done()]) > workers:   # bound the host copies held for writing
+                    next(w for w in writes if not w.done()).result()
+            for w in writes:
+                w.result()
+
+
+def _read_case(image_files, seg_file, plans_manager):
+    """The case as the plans' reader delivers it: (images, seg or None, properties)."""
+    rw = plans_manager.image_reader_writer_class()
+    data, data_properties = rw.read_images(image_files)
+    seg = rw.read_seg(seg_file)[0] if seg_file is not None else None
+    return data, seg, data_properties
+
+
+def _save_case(output_filename_truncated: str, data: np.ndarray, seg: np.ndarray, properties: dict):
+    np.savez_compressed(output_filename_truncated + ".npz", data=data, seg=seg)
+    with open(output_filename_truncated + ".pkl", "wb") as f:
+        pickle.dump(properties, f)
+
+
+# ---- the host nnU-Net's dataset helpers, which the dataset loops are called from (tests substitute them) -------------
+
+
+def _dataset_name(dataset_name_or_id) -> str:
+    from dinounet.utilities.dataset_name_id_conversion import maybe_convert_to_dataset_name
+    return maybe_convert_to_dataset_name(dataset_name_or_id)
+
+
+def _raw_and_preprocessed():
+    """(nnUNet_raw, nnUNet_preprocessed)."""
+    from dinounet import paths
+    return paths.nnUNet_raw, paths.nnUNet_preprocessed
+
+
+def _plans_manager(plans: dict):
+    from dinounet.utilities.plans_handling.plans_handler import PlansManager
+    return PlansManager(plans)
+
+
+def _get_filenames_of_train_images_and_targets(raw_dataset_folder: str, dataset_json: dict) -> dict:
+    from dinounet.utilities.utils import get_filenames_of_train_images_and_targets
+    return get_filenames_of_train_images_and_targets(raw_dataset_folder, dataset_json)
 
 
 def memory_axes(data) -> list:

@@ -278,6 +278,29 @@ int b2u_pre_seg_compact(const void* seg, int32_t dtype, int64_t n, const int64_t
 int b2u_pre_seg_gather(const int32_t* idx, const int64_t* ranks, int64_t t, int32_t H, int32_t W, int64_t* rows,
                        b2u_stream_t stream);
 
+/* ---- Dataset fingerprint (experiment_planning/dataset_fingerprint/fingerprint_extractor.py:41-80 and 156-184).
+ * b2u_fp_fg_compact: idx (DEVICE int32 [n]) = the ascending linear indices of the voxels with seg > 0 (the seg in its
+ *   stored dtype, B2U_EVAL_* code; a NaN voxel is not foreground); *count (DEVICE int64) = their number.  n < 2^31.
+ *   work: b2u_pre_seg_compact_work_ints(n) int32.
+ * b2u_fp_gather: out[c * out_stride + j] = img[c * n_vox + idx[ranks[c * m + j]]] for c < C, j < m (img: DEVICE fp32
+ *   [C, n_vox]; ranks: DEVICE int64 [C, m], or null for idx[j]).
+ * b2u_fp_select: out (DEVICE fp32 [R]) = the values at the 0-based ranks (HOST int64 [R], 1 <= R <= B2U_FP_MAX_RANKS,
+ *   each in [0, n)) of x (DEVICE fp32 [n]) in ascending order, exact; -0.0 and +0.0 are equal and returned as +0.0.
+ *   work: b2u_fp_select_work_bytes() bytes (DEVICE).
+ * b2u_fp_moments: stats = numpy's mean and (with_std) std of x [n]: float32 stats (DEVICE fp32 [2]), or with f64 the
+ *   float64 statistics of x converted to float64 (DEVICE fp64 [2]).  work: b2u_fp_moments_work_bytes(n, f64) bytes. */
+#define B2U_FP_MAX_RANKS 8
+int b2u_fp_fg_compact(const void* seg, int32_t dtype, int64_t n, int32_t* work, int32_t* idx, int64_t* count,
+                      b2u_stream_t stream);
+int b2u_fp_gather(const float* img, int32_t C, int64_t n_vox, const int32_t* idx, const int64_t* ranks, int64_t m,
+                  float* out, int64_t out_stride, b2u_stream_t stream);
+int64_t b2u_fp_select_work_bytes(void);
+int b2u_fp_select(const float* x, int64_t n, const int64_t* ranks, int32_t R, void* work, float* out,
+                  b2u_stream_t stream);
+int64_t b2u_fp_moments_work_bytes(int64_t n, int32_t f64);
+int b2u_fp_moments(const float* x, int64_t n, int32_t f64, int32_t with_std, void* work, void* stats,
+                   b2u_stream_t stream);
+
 /* ---- Evaluation of predictions against the ground truth (evaluation/evaluate_predictions.py:152-230
  * `compute_metrics`, HD95 / ASD as medpy's hd95 / asd).  Volumes are C-contiguous [Z, Y, X] (a mask of rank 1 or 2 is
  * padded with leading axes of size 1, and `ndim` names its true rank).
