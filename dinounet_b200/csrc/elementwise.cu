@@ -640,25 +640,32 @@ extern "C" int b2u_tail_fuse(const void* base, int32_t base_fp32, int64_t base_b
 }
 
 // ------------------------------------------------------------------------------------------------ InstanceNorm
-// stats: block = (row chunk, image b); thread = (row lane, 8-channel group); smem tree over row lanes; the block's
-// partial (shifted sum, shifted sumsq) per channel goes to a workspace slot, and the LAST block of each image (ticket counter)
-// adds the slots in fixed chunk order -> bitwise deterministic, no float atomics, no zero-fill of `sums` needed.
-// Output per (image, channel): (sum x, sum (x - mean)^2).
+// stats: block = (row chunk, image b); thread = (row lane, 8-channel group); smem tree over row lanes.  Each block makes two
+// passes over its chunk (the second from L2): the chunk sum, then the sum of squares about the chunk's own mean.  The block's
+// partial (sum, centred sumsq) per channel goes to a workspace slot, and the LAST block of each image (ticket counter)
+// merges the slots in fixed chunk order (Chan et al.'s pairwise update) -> bitwise deterministic, no float atomics, no
+// zero-fill of `sums` needed.  Output per (image, channel): (sum x, sum (x - mean)^2).
+// Workspace: kInTickets ticket counters, then the partials.  The partials start at the same offset for every (B, rows, C),
+// so one workspace can serve calls of different shapes: partials of one call never land on another call's counters.
+constexpr int kInTickets = 1024;
 static inline int in_stats_chunk(int rows) { return rows >= 8192 ? 2048 : (rows >= 1024 ? 256 : 64); }
 
 template <typename T>
 __global__ void __launch_bounds__(256) in_stats_kernel(const T* __restrict__ x, long long ldx, float* __restrict__ sums,
                                                        float* __restrict__ work, int rows, int C8, int chunk) {
   pdl_begin();
-  extern __shared__ float red[];  // [rows_par][C8*16]
+  extern __shared__ float red[];  // [rows_par][C8*16], then the chunk sums [C8*8]
   __shared__ int s_last;
   const int b = blockIdx.y, nchunks = gridDim.x, B = gridDim.y;
   const int cg = threadIdx.x % C8, rl = threadIdx.x / C8;
   const int rows_par = 256 / C8;
   const int r0 = blockIdx.x * chunk;
   const int r1 = min(rows, r0 + chunk);
-  // Shifted sums: every block of image b accumulates sum(x - x0) and sum((x - x0)^2) with x0 = the image's first pixel of the
-  // channel, so the variance below never subtracts two large nearly equal numbers when |mean| >> std
+  const int nout = C8 * 16;  // per image: C channels x (sum, sumsq), laid out [cg][k][j]
+  float* csum = red + rows_par * nout;
+  // Sums are taken of x - x0 (x0 = the image's first pixel of the channel) so that they stay small when |mean| >> std.
+  // The squares are taken about the chunk mean, not about x0: a first pixel far from the mean (a padded border, a hot
+  // pixel) would otherwise leave the variance as the difference of two large, nearly equal sums.
   float sh[8];
   {
     Vec8<T> v0;
@@ -672,15 +679,36 @@ __global__ void __launch_bounds__(256) in_stats_kernel(const T* __restrict__ x, 
     float f[8];
     v.to_float(f);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) { const float d = f[j] - sh[j]; s[j] += d; q[j] = fmaf(d, d, q[j]); }
+    for (int j = 0; j < 8; ++j) s[j] += f[j] - sh[j];
   }
   float* my = red + (rl * C8 + cg) * 16;
 #pragma unroll
-  for (int j = 0; j < 8; ++j) { my[j] = s[j]; my[8 + j] = q[j]; }
+  for (int j = 0; j < 8; ++j) my[j] = s[j];
   __syncthreads();
-  const int nout = C8 * 16;  // per image: C channels x (sum, sumsq), laid out [cg][k][j]
+  for (int o = threadIdx.x; o < C8 * 8; o += 256) {
+    const int g = o >> 3, j = o & 7;
+    float t = 0.f;
+    for (int p = 0; p < rows_par; ++p) t += red[p * nout + g * 16 + j];
+    csum[o] = t;
+  }
+  __syncthreads();
+  float mc[8];
+  const float inv_n = 1.f / static_cast<float>(r1 - r0);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) mc[j] = csum[cg * 8 + j] * inv_n;
+  for (int r = r0 + rl; r < r1; r += rows_par) {
+    Vec8<T> v;
+    v.load(x + (static_cast<long long>(b) * rows + r) * ldx + cg * 8);
+    float f[8];
+    v.to_float(f);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) { const float d = (f[j] - sh[j]) - mc[j]; q[j] = fmaf(d, d, q[j]); }
+  }
+#pragma unroll
+  for (int j = 0; j < 8; ++j) my[8 + j] = q[j];
+  __syncthreads();
   int* counters = reinterpret_cast<int*>(work);
-  float* part = work + B + (static_cast<long long>(b) * nchunks + blockIdx.x) * nout;
+  float* part = work + kInTickets + (static_cast<long long>(b) * nchunks + blockIdx.x) * nout;
   for (int o = threadIdx.x; o < nout; o += 256) {
     float t = 0.f;
     for (int p = 0; p < rows_par; ++p) t += red[p * nout + o];
@@ -692,25 +720,28 @@ __global__ void __launch_bounds__(256) in_stats_kernel(const T* __restrict__ x, 
   __syncthreads();
   if (!s_last) return;
   __threadfence();
-  const float* pb = work + B + static_cast<long long>(b) * nchunks * nout;
+  const float* pb = work + kInTickets + static_cast<long long>(b) * nchunks * nout;
   for (int o = threadIdx.x; o < C8 * 8; o += 256) {       // one thread per channel: fixed chunk order -> deterministic
     const int g = o >> 3, j = o & 7;
     float ts = 0.f, tq = 0.f;
-    for (int c = 0; c < nchunks; ++c) {
-      ts += __ldcg(pb + static_cast<long long>(c) * nout + g * 16 + j);
-      tq += __ldcg(pb + static_cast<long long>(c) * nout + g * 16 + 8 + j);
+    for (int c = 0; c < nchunks; ++c) ts += __ldcg(pb + static_cast<long long>(c) * nout + g * 16 + j);
+    const float md = ts / static_cast<float>(rows);
+    for (int c = 0; c < nchunks; ++c) {   // M2 = sum_c [M2_c + n_c (mean_c - mean)^2]
+      const float n_c = static_cast<float>(min(chunk, rows - c * chunk));
+      const float dm = __ldcg(pb + static_cast<long long>(c) * nout + g * 16 + j) / n_c - md;
+      tq += fmaf(n_c * dm, dm, __ldcg(pb + static_cast<long long>(c) * nout + g * 16 + 8 + j));
     }
     const float x0 = T16<T>::to_f(x[static_cast<long long>(b) * rows * ldx + o]);
     float* dst = sums + (static_cast<long long>(b) * C8 * 8 + o) * 2;
     dst[0] = fmaf(static_cast<float>(rows), x0, ts);                  // sum x
-    dst[1] = fmaxf(tq - ts * ts / static_cast<float>(rows), 0.f);     // sum (x - mean)^2
+    dst[1] = tq;                                                      // sum (x - mean)^2
   }
   if (threadIdx.x == 0) counters[b] = 0;  // self-resetting ticket
 }
 
 extern "C" int64_t b2u_in_stats_work_floats(int32_t B, int32_t rows, int32_t C) {
   const int chunk = in_stats_chunk(rows);
-  return static_cast<int64_t>(B) + static_cast<int64_t>(B) * ((rows + chunk - 1) / chunk) * C * 2;
+  return static_cast<int64_t>(kInTickets) + static_cast<int64_t>(B) * ((rows + chunk - 1) / chunk) * C * 2;
 }
 
 extern "C" int b2u_in_stats(const void* x, int64_t ldx, float* sums, float* work, int32_t B, int32_t rows, int32_t C,
@@ -718,10 +749,11 @@ extern "C" int b2u_in_stats(const void* x, int64_t ldx, float* sums, float* work
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (C % 8 || C > 2048 || (256 % (C / 8))) return set_error(-1, "b2u_in_stats: C must be 8*2^k <= 2048");
   if (!work) return set_error(-1, "b2u_in_stats: workspace required");
+  if (B > kInTickets) return set_error(-1, "b2u_in_stats: B > %d", kInTickets);
   const int C8 = C / 8;
   const int chunk = in_stats_chunk(rows);
   dim3 grid((rows + chunk - 1) / chunk, B);
-  const size_t smem = static_cast<size_t>(256 / C8) * C8 * 16 * sizeof(float);
+  const size_t smem = (static_cast<size_t>(256 / C8) * C8 * 16 + C8 * 8) * sizeof(float);
   B2U_DISPATCH_T(dtype, (launch_pdl(in_stats_kernel<T>, grid, 256, smem, stream, static_cast<const T*>(x), ldx, sums, work, rows, C8, chunk)));
   return check_launch("in_stats");
 }

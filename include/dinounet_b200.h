@@ -415,11 +415,13 @@ int b2u_tail_fuse(const void* base, int32_t base_fp32, int64_t base_batch_stride
                   const float* scale, const float* shift, int32_t B, int32_t H, int32_t W, int32_t Ht, int32_t Wt,
                   int32_t D, int32_t dtype, b2u_stream_t stream);
 
-/* InstanceNorm statistics: sums[b, c, 0..1] = (sum x, sum (x - mean)^2) over the rows of image b (accumulated as shifted
- * sums around the image's first pixel: no cancellation when |mean| >> std).  x 16-bit [B*rows, C] with row
- * stride ldx (dinounet_training.py:400-401; ConvDropoutNormReLU norm).  Deterministic two-level reduction (no float
- * atomics): `work` holds >= b2u_in_stats_work_floats(B, rows, C) floats whose first B words are ticket counters that
- * must be ZERO before the first call (the kernel leaves them zero); a workspace may be shared by consecutive calls. */
+/* InstanceNorm statistics: sums[b, c, 0..1] = (sum x, sum (x - mean)^2) over the rows of image b (sums shifted by the
+ * image's first pixel, squares taken about each row chunk's own mean and merged pairwise: no cancellation when
+ * |mean| >> std or when the first pixel is far from the mean).  x 16-bit [B*rows, C] with row stride ldx
+ * (dinounet_training.py:400-401; ConvDropoutNormReLU norm), B <= 1024.  Deterministic two-level reduction (no float
+ * atomics): `work` holds >= b2u_in_stats_work_floats(B, rows, C) floats whose first 1024 words are ticket counters that
+ * must be ZERO before the first call (the kernel leaves them zero); a workspace may be shared by consecutive calls of
+ * any shapes it is large enough for. */
 int64_t b2u_in_stats_work_floats(int32_t B, int32_t rows, int32_t C);
 int b2u_in_stats(const void* x, int64_t ldx, float* sums, float* work, int32_t B, int32_t rows, int32_t C, int32_t dtype,
                  b2u_stream_t stream);
