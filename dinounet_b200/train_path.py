@@ -686,60 +686,104 @@ def all_reduce_gradients(params, group=None, average: bool = True):
         off += n
 
 
-class FusedSGD:
+class FusedSGD(torch.optim.Optimizer):
     """torch.optim.SGD(lr, weight_decay, momentum 0.99, nesterov=True) + clip_grad_norm_(12) (nnUNetTrainer.py:486-489,
     922-923) on the hand-written kernels: one squared-norm reduction per tensor into a device scalar, then one fused update
-    per tensor that reads the clip coefficient from device memory (no host synchronisation).  `param_groups[0]["lr"]` is
-    what the reference's PolyLRScheduler writes (training/lr_scheduler/polylr.py)."""
+    per tensor that reads the clip coefficient from device memory (no host synchronisation).
+
+    A `torch.optim.Optimizer`: the reference's PolyLRScheduler (training/lr_scheduler/polylr.py) and torch's schedulers
+    construct on it and write `param_groups[i]["lr"]`.  Every parameter given stays in its group, in order, frozen ones
+    included, as `torch.optim.SGD(network.parameters())` keeps them; a parameter without a gradient is skipped, and its
+    momentum buffer is created the first time it has one (torch's first-step rule: buffer = gradient).  `state_dict()` /
+    `load_state_dict()` use torch.optim.SGD's format, so a checkpoint of either optimizer resumes on the other.  The clip
+    threshold `max_norm` is a constructor argument on both sides and not part of the state."""
 
     def __init__(self, params, lr: float, weight_decay: float = 3e-5, momentum: float = 0.99, max_norm: float = 12.0):
-        self.params = [p for p in params if p.requires_grad]
-        self.param_groups = [{"params": self.params, "lr": lr, "weight_decay": weight_decay, "momentum": momentum, "nesterov": True}]
+        # torch.optim.SGD's group keys, so that the state dicts of the two optimizers are interchangeable
+        defaults = dict(lr=lr, momentum=momentum, dampening=0, weight_decay=weight_decay, nesterov=True, maximize=False,
+                        foreach=None, differentiable=False, fused=None)
+        super().__init__(params, defaults)
         self.max_norm = max_norm
-        self.bufs = [torch.zeros_like(p) for p in self.params]
-        self.first = True
         self._sq = None
 
-    lr = property(lambda self: self.param_groups[0]["lr"])
-    wd = property(lambda self: self.param_groups[0]["weight_decay"])
-    mom = property(lambda self: self.param_groups[0]["momentum"])
+    @property
+    def params(self) -> List[torch.Tensor]:
+        return [p for group in self.param_groups for p in group["params"]]
+
+    def load_state_dict(self, state_dict: dict) -> None:
+        """torch.optim.SGD's state dict (`state`: index -> {"momentum_buffer"}, `param_groups` with the index lists).
+        ValueError for another parameter count or a buffer shaped unlike its parameter; NotImplementedError for the
+        settings the fused update does not compute (nesterov=False, dampening != 0, maximize)."""
+        groups, saved = self.param_groups, state_dict["param_groups"]
+        if len(groups) != len(saved) or any(len(g["params"]) != len(s["params"]) for g, s in zip(groups, saved)):
+            raise ValueError(f"optimizer state holds {[len(s['params']) for s in saved]} parameters per group, this "
+                             f"optimizer {[len(g['params']) for g in groups]}")
+        for s in saved:
+            if not s.get("nesterov", False) or s.get("dampening", 0) != 0 or s.get("maximize", False):
+                raise NotImplementedError("FusedSGD computes SGD with nesterov=True, dampening=0 and maximize=False; the "
+                                          f"state has nesterov={s.get('nesterov')}, dampening={s.get('dampening')}, "
+                                          f"maximize={s.get('maximize')}")
+        index_to_param = {i: p for s, g in zip(saved, groups) for i, p in zip(s["params"], g["params"])}
+        for i, st in state_dict["state"].items():
+            if i not in index_to_param:
+                raise ValueError(f"optimizer state has an entry for parameter {i}, which no parameter group lists")
+            buf = st.get("momentum_buffer")
+            if buf is not None and tuple(buf.shape) != tuple(index_to_param[i].shape):
+                raise ValueError(f"momentum buffer {i} has shape {tuple(buf.shape)}, its parameter "
+                                 f"{tuple(index_to_param[i].shape)}")
+        super().load_state_dict(state_dict)
+        for p in self.params:   # the update kernel reads dense buffers; torch.optim.SGD stores None for no buffer
+            st = self.state.get(p)
+            if st is not None and st.get("momentum_buffer") is None:
+                del self.state[p]
+            elif st is not None:
+                st["momentum_buffer"] = st["momentum_buffer"].contiguous()
 
     @torch.no_grad()
-    def step(self):
+    def step(self, closure=None):
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
         ps = [p for p in self.params if p.grad is not None]
         if not ps:
-            return
+            return loss
         dev = ps[0].device
         if self._sq is None:
             self._sq = torch.zeros(1, dtype=torch.float64, device=dev)
         self._sq.zero_()
         for p in ps:
             _call("b2u_f32_sqsum", p.grad.contiguous(), p.numel(), self._sq)
-        for p, buf in zip(self.params, self.bufs):
-            if p.grad is None:
-                continue
-            g = p.grad.contiguous()
-            with torch.cuda.device(dev):
-                L.check(L.load().b2u_f32_sgd_nesterov(p.data_ptr(), g.data_ptr(), buf.data_ptr(), p.numel(), self.lr, self.mom, self.wd,
-                                                      self._sq.data_ptr(), self.max_norm, 1 if self.first else 0,
-                                                      C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "sgd")
-        self.first = False
+        lib = L.load()
+        with torch.cuda.device(dev):
+            stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            for group in self.param_groups:
+                for p in group["params"]:
+                    if p.grad is None:
+                        continue
+                    g = p.grad.contiguous()
+                    st = self.state[p]
+                    first = "momentum_buffer" not in st
+                    if first:   # the kernel writes the buffer without reading it on a first step
+                        st["momentum_buffer"] = torch.empty_like(p, memory_format=torch.contiguous_format)
+                    L.check(lib.b2u_f32_sgd_nesterov(p.data_ptr(), g.data_ptr(), st["momentum_buffer"].data_ptr(), p.numel(),
+                                                     group["lr"], group["momentum"], group["weight_decay"],
+                                                     self._sq.data_ptr(), self.max_norm, 1 if first else 0, stream), "sgd")
+        return loss
 
     def grad_norm(self) -> float:
         return float(self._sq.sqrt().item())
-
-    def zero_grad(self, set_to_none: bool = True):
-        for p in self.params:
-            p.grad = None
 
 
 def train_step(net, loss_fn, optimizer: FusedSGD, data: torch.Tensor, target: torch.Tensor, group=None) -> torch.Tensor:
     """One optimisation step with the semantics of `nnUNetTrainer.train_step` (nnUNetTrainer.py:899-929): zero grads,
     forward, Dice+CE, backward, (data-parallel: one gradient all-reduce), clip 12, SGD-nesterov.  fp32 end to end outside the
-    frozen ViT (no GradScaler: there is no fp16 gradient to scale).  Returns the detached loss."""
+    frozen ViT (no GradScaler: there is no fp16 gradient to scale).  The step changes the weights in place, so the next
+    eval-path entry of `net` (a validation forward) repacks its engine.  Returns the detached loss."""
     optimizer.zero_grad()
     loss = loss_fn(net(data), target)
     loss.backward()
     all_reduce_gradients(optimizer.params, group)
     optimizer.step()
+    net._repack_before_eval = True
     return loss.detach()

@@ -6,10 +6,14 @@ planner's architecture dict on the class, and the static `build_network_architec
 trainers derive from its `nnUNetTrainerNoDeepSupervision`, so `api.training(trainer_class=DinoUNetTrainer_l, ...)`
 works unchanged; otherwise they derive from `object` (the hook itself is a staticmethod and needs no base class).
 """
+import os
+import warnings
+from concurrent.futures import ThreadPoolExecutor
 from typing import List, Tuple, Union
 
 import numpy as np
 import torch
+from torch import distributed as dist
 from torch import nn
 
 from . import config as cfg
@@ -119,15 +123,15 @@ class DinoUNetTrainer(_Base):
     # ---- training step on the native path (nnUNetTrainer.py:486-489, 899-929)
     def configure_optimizers(self):
         """SGD(momentum 0.99, nesterov, weight decay) + the reference's PolyLRScheduler (it only writes param_groups[0]['lr'])
-        on the fused kernels; gradient clipping (12) is part of the fused step."""
+        on the fused kernels; gradient clipping (12) is part of the fused step.  Without the reference package there is
+        no scheduler; a scheduler that fails to construct raises."""
         from .train_path import FusedSGD
         optimizer = FusedSGD(self.network.parameters(), self.initial_lr, weight_decay=self.weight_decay, momentum=0.99, max_norm=12.0)
         try:
             from dinounet.training.lr_scheduler.polylr import PolyLRScheduler
-            lr_scheduler = PolyLRScheduler(optimizer, self.initial_lr, self.num_epochs)
-        except Exception:  # pragma: no cover - reference stack absent
-            lr_scheduler = None
-        return optimizer, lr_scheduler
+        except ImportError:  # pragma: no cover - reference stack absent
+            return optimizer, None
+        return optimizer, PolyLRScheduler(optimizer, self.initial_lr, self.num_epochs)
 
     def train_step(self, batch: dict) -> dict:
         from .train_path import train_step
@@ -154,6 +158,98 @@ class DinoUNetTrainer(_Base):
             output = self.network(data)
         del data
         return validation_statistics(self.loss, output, target)
+
+    # ---- final validation on the device (nnUNetTrainer.py:1146-1293)
+    def _validation_keys(self):
+        """`do_split()`'s validation keys, under DDP this rank's share `val_keys[rank::world]`, and the last case index
+        after which the periodic barrier stops (every rank reaches it), as nnUNetTrainer.py:1174-1180."""
+        _, val_keys = self.do_split()
+        last_barrier_at_idx = None
+        if self.is_ddp:
+            world = dist.get_world_size()
+            last_barrier_at_idx = len(val_keys) // world - 1
+            val_keys = val_keys[self.local_rank::world]
+        return val_keys, last_barrier_at_idx
+
+    def perform_actual_validation(self, save_probabilities: bool = False):
+        """The validation at the end of training on the device: each validation case is predicted by
+        `SlidingWindowPredictor` (tile step 0.5, gaussian, no mirroring) on the network's current weights, and its fp16
+        logits go to the device export without leaving the GPU.  `VALIDATION_WRITERS` threads run the export, with at
+        most two cases queued beyond them: its kernels and its copy of the labels to the host are ordered after the
+        prediction work already queued on the stream, and its host part (geometry, file writing) overlaps the next
+        case's prediction.  Rank 0 then scores `validation/` against `gt_segmentations/` with the device evaluation into
+        `validation/summary.json`.  The cascade and next-stage predictions are not implemented: they raise before
+        anything runs."""
+        from . import evaluation, export
+        from .sliding_window import SlidingWindowPredictor
+        if self.is_cascaded:
+            raise NotImplementedError("the final validation on the device does not implement the cascade")
+        if self.configuration_manager.next_stage_names is not None:
+            raise NotImplementedError("the final validation on the device does not predict for next stages "
+                                      f"({self.configuration_manager.next_stage_names})")
+        self.network.eval()
+        net = self.network.module if self.is_ddp else self.network
+        net.repack()   # the optimizer changed the weights in place since the engine packed them
+        predictor = SlidingWindowPredictor(tile_step_size=0.5, use_gaussian=True, use_mirroring=False,
+                                           perform_everything_on_device=True, device=self.device)
+        predictor.manual_initialization(net, self.plans_manager, self.configuration_manager, None, self.dataset_json,
+                                        self.__class__.__name__, self.inference_allowed_mirroring_axes)
+        validation_output_folder = os.path.join(self.output_folder, "validation")
+        os.makedirs(validation_output_folder, exist_ok=True)
+        val_keys, last_barrier_at_idx = self._validation_keys()
+        dataset_val = _validation_dataset(self.preprocessed_dataset_folder, val_keys,
+                                          self.folder_with_segs_from_previous_stage)
+        # the writers enqueue the export on the stream the logits were computed on
+        stream = torch.cuda.current_stream(predictor.device if predictor.device.index is not None else None)
+
+        def write(logits, properties, output_filename_truncated):
+            with torch.cuda.stream(stream):
+                export.export_prediction_from_logits(logits, properties, self.configuration_manager, self.plans_manager,
+                                                     self.dataset_json, output_filename_truncated, save_probabilities)
+
+        with ThreadPoolExecutor(VALIDATION_WRITERS) as writers:
+            pending = []
+            for i, k in enumerate(dataset_val.keys()):
+                while len(pending) >= VALIDATION_WRITERS + 2:   # allowed_num_queued=2 (nnUNetTrainer.py:1194-1199)
+                    pending.pop(0).result()
+                self.print_to_log_file(f"predicting {k}")
+                data, _, properties = dataset_val.load_case(k)
+                with warnings.catch_warnings():
+                    warnings.simplefilter("ignore")   # 'The given NumPy array is not writable'
+                    data = torch.from_numpy(data)
+                self.print_to_log_file(f"{k}, shape {data.shape}, rank {self.local_rank}")
+                logits = predictor.predict_sliding_window_return_logits(data)
+                pending.append(writers.submit(write, logits, properties, os.path.join(validation_output_folder, k)))
+                del logits
+                if self.is_ddp and i < last_barrier_at_idx and (i + 1) % 20 == 0:
+                    dist.barrier()
+            for f in pending:
+                f.result()
+        if self.is_ddp:
+            dist.barrier()
+        if self.local_rank == 0:
+            lm = self.label_manager
+            metrics = evaluation.compute_metrics_on_folder(
+                os.path.join(self.preprocessed_dataset_folder_base, "gt_segmentations"), validation_output_folder,
+                os.path.join(validation_output_folder, "summary.json"), self.plans_manager.image_reader_writer_class(),
+                self.dataset_json["file_ending"], lm.foreground_regions if lm.has_regions else lm.foreground_labels,
+                lm.ignore_label, chill=True,
+                num_processes=evaluation.DEFAULT_NUM_PROCESSES * (dist.get_world_size() if self.is_ddp else 1))
+            self.print_to_log_file("Validation complete", also_print_to_console=True)
+            self.print_to_log_file("Mean Validation Dice: ", (metrics["foreground_mean"]["Dice"]),
+                                   also_print_to_console=True)
+
+
+#: threads that export and write the final validation's cases; their host work overlaps the next prediction
+VALIDATION_WRITERS = 2
+
+
+def _validation_dataset(folder: str, keys, folder_with_segs_from_previous_stage):
+    """The reference's dataset of preprocessed cases (`<key>.npz` / `<key>.pkl`), loaded with `load_case(key)` ->
+    (data, seg, properties).  Tests substitute it."""
+    from dinounet.training.dataloading.nnunet_dataset import nnUNetDataset
+    return nnUNetDataset(folder, keys, folder_with_segs_from_previous_stage=folder_with_segs_from_previous_stage,
+                         num_images_properties_loading_threshold=0)
 
 
 class PassThroughTransforms:

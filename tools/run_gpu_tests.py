@@ -11,7 +11,7 @@ ap.add_argument("-k", default="")
 ap.add_argument("--timeout", type=int, default=240)
 ap.add_argument("--per-test", action="store_true")
 ap.add_argument("--files", nargs="*", default=["tests/test_gpu_kernels.py", "tests/test_gpu_parity.py", "tests/test_gpu_sliding_window.py",
-                                          "tests/test_gpu_loss.py"])
+                                          "tests/test_gpu_loss.py", "tests/test_gpu_trainer_loop.py"])
 a = ap.parse_args()
 os.makedirs("gpurun_out", exist_ok=True)
 cmd = [sys.executable, "-m", "pytest", "--collect-only", "-q", "-m", "gpu", *a.files]
