@@ -279,6 +279,8 @@ __global__ void f32_seg_out_kernel(const float* __restrict__ lin, float* __restr
 }
 extern "C" int b2u_f32_seg_out(const float* lin, float* logits, uint8_t* labels, int32_t B, int64_t HW, int32_t ncls,
                                b2u_stream_t stream_) {
+  // labels are uint8: class 255 is the largest one they hold
+  if (ncls < 1 || ncls > 256) return set_error(-1, "b2u_f32_seg_out: 1 <= ncls <= 256");
   const long long total = static_cast<long long>(B) * HW;
   f32_seg_out_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream_)>>>(lin, logits, labels, B, HW, ncls);
   return check_launch("f32_seg_out");
