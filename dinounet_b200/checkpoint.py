@@ -21,9 +21,18 @@ def load_network_weights(network: torch.nn.Module, filename_or_checkpoint: Union
         ckpt = torch.load(ckpt, map_location="cpu", weights_only=False)     # the reference pickles plain python objects too
     if "network_weights" not in ckpt:
         raise KeyError("not an nnU-Net checkpoint: no 'network_weights' entry")
-    own = set(network.state_dict().keys())
+    weights = match_keys(ckpt["network_weights"], set(network.state_dict().keys()))
+    network.load_state_dict(weights, strict=strict)
+    if hasattr(network, "repack"):
+        network.repack()          # packed K-major kernel weights are rebuilt on the next forward
+    return {k: ckpt.get(k) for k in ("trainer_name", "init_args", "current_epoch", "inference_allowed_mirroring_axes")}
+
+
+def match_keys(network_weights: dict, own: set) -> dict:
+    """The checkpoint's weights under the network's own keys: a key the network lacks loses a DataParallel /
+    torch.compile prefix when that names one of the network's keys."""
     weights = {}
-    for k, v in ckpt["network_weights"].items():
+    for k, v in network_weights.items():
         key = k
         if key not in own:
             for p in _PREFIXES:
@@ -31,7 +40,4 @@ def load_network_weights(network: torch.nn.Module, filename_or_checkpoint: Union
                     key = key[len(p):]
                     break
         weights[key] = v
-    network.load_state_dict(weights, strict=strict)
-    if hasattr(network, "repack"):
-        network.repack()          # packed K-major kernel weights are rebuilt on the next forward
-    return {k: ckpt.get(k) for k in ("trainer_name", "init_args", "current_epoch", "inference_allowed_mirroring_axes")}
+    return weights

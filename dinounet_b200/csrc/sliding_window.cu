@@ -29,7 +29,8 @@ __global__ void sw_gather_kernel(const float* __restrict__ vol, float* __restric
 
 __device__ __forceinline__ float h_round(float v) { return __half2float(__float2half_rn(v)); }
 
-// One tile: entries first..first+nvar-1 of `logits` are its mirror variants (variant 0 unflipped).
+// One tile: entries first..first+nvar-1 of `logits` are its mirror variants (variant 0 unflipped).  npred == nullptr:
+// accumulate the logits only (the other folds of an ensemble share one weight count).
 __global__ void sw_accumulate_kernel(const float* __restrict__ logits, const int32_t* __restrict__ desc, int first,
                                      int nvar, const __half* __restrict__ gauss, __half* __restrict__ acc,
                                      __half* __restrict__ npred, int C, int D, int H, int W, int th, int tw) {
@@ -55,7 +56,7 @@ __global__ void sw_accumulate_kernel(const float* __restrict__ logits, const int
     const long long o = c * cstride + pix;
     acc[o] = __float2half_rn(__half2float(acc[o]) + pg);
   }
-  npred[pix] = __float2half_rn(__half2float(npred[pix]) + g);
+  if (npred) npred[pix] = __float2half_rn(__half2float(npred[pix]) + g);
 }
 
 __global__ void sw_finalize_kernel(__half* __restrict__ acc, const __half* __restrict__ npred, int C, long long plane,
@@ -88,7 +89,7 @@ extern "C" int b2u_sw_accumulate(const float* logits, const int32_t* tile_desc, 
                                  const void* gaussian, void* acc, void* npred, int32_t C, int32_t D, int32_t H,
                                  int32_t W, int32_t th, int32_t tw, b2u_stream_t stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (!logits || !tile_desc || !acc || !npred) return set_error(-1, "b2u_sw_accumulate: null pointer");
+  if (!logits || !tile_desc || !acc) return set_error(-1, "b2u_sw_accumulate: null pointer");
   if (nvar != 1 && nvar != 2 && nvar != 4) return set_error(-1, "b2u_sw_accumulate: nvar %d not in {1,2,4}", nvar);
   sw_accumulate_kernel<<<(th * tw + 255) / 256, 256, 0, stream>>>(
       logits, tile_desc, first, nvar, static_cast<const __half*>(gaussian), static_cast<__half*>(acc),

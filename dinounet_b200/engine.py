@@ -17,8 +17,10 @@ from __future__ import annotations
 
 import ctypes as C
 import math
+import threading
 from collections import OrderedDict
-from typing import Dict, List, Optional, Tuple
+from contextlib import contextmanager
+from typing import Dict, Iterable, List, Optional, Tuple
 
 import torch
 
@@ -39,6 +41,47 @@ def _patch_qkv_rope(args, sin: int, cos: int, keep: list):
     qp.rope_sin, qp.rope_cos = sin, cos
     keep.append(qp)
     return (C.byref(qp),)
+
+
+class _CaptureGuard:
+    """Keeps other threads' device work out of CUDA graph captures.  A capture in CUDA's default (global) mode fails,
+    together with the caller, when another thread makes a call that is not allowed during a capture (an allocation, a
+    synchronisation).  Threads that run device work beside the engine (the prediction's export writers) do it inside
+    `device_work()`; a capture waits until none of them is inside and keeps new ones out until it ends."""
+
+    def __init__(self):
+        self._cv = threading.Condition()
+        self._workers = 0
+        self._capturing = False
+
+    @contextmanager
+    def capture(self):
+        with self._cv:
+            self._cv.wait_for(lambda: not self._capturing)
+            self._capturing = True
+            self._cv.wait_for(lambda: self._workers == 0)
+        try:
+            yield
+        finally:
+            with self._cv:
+                self._capturing = False
+                self._cv.notify_all()
+
+    @contextmanager
+    def device_work(self):
+        with self._cv:
+            self._cv.wait_for(lambda: not self._capturing)
+            self._workers += 1
+        try:
+            yield
+        finally:
+            with self._cv:
+                self._workers -= 1
+                self._cv.notify_all()
+
+
+#: the process's guard around every graph capture of the engines (see `_CaptureGuard`)
+GRAPH_CAPTURE = _CaptureGuard()
 
 
 class Plan:
@@ -110,6 +153,10 @@ class ForwardEngine:
         self._plans: "OrderedDict[Tuple[int, int], Tuple[Plan, dict]]" = OrderedDict()
         self._graphs: Dict[Tuple[int, int], object] = {}
         self.max_plans = 4
+        # fold weight sets (`pack_folds`): the packed weights after the taps of each fold of a run whose folds share this
+        # engine's backbone, and per (B, S) one "rest" launch list per fold on that plan's buffers
+        self._folds: List[Dict[str, torch.Tensor]] = []
+        self._fold_plans: Dict[Tuple[int, int], List[Plan]] = {}
         if self.device.type != "cuda":
             raise L.NativeLibraryError("dinounet_b200 runs on CUDA devices only (no CPU fallback)")
         with torch.cuda.device(self.device):
@@ -143,11 +190,21 @@ class ForwardEngine:
 
     def pack(self, P: Dict[str, torch.Tensor]):
         """(Re)build the kernel-native weight copies from a reference-keyed state dict."""
+        w = self._pack_vit(P)
+        w.update(self._pack_rest(P))
+        self.w = w
+        self._plans.clear()
+        self._graphs.clear()
+        self._folds = []
+        self._fold_plans.clear()
+
+    def _pack_vit(self, P: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+        """The frozen backbone's packed weights (patch embed .. final norm): what the plan's ViT section reads."""
         v, w = self.v, {}
         D = v.embed_dim
         A = "encoder.dinov3_adapter."
         Bk = A + "backbone."
-        tv, tr = self.tv, self.tr
+        tv = self.tv
         f32 = self._dev
         # ---- ViT
         w["pe.w"] = self._lin(P[Bk + "patch_embed.proj.weight"], tv)
@@ -175,6 +232,15 @@ class ForwardEngine:
                                                    P[p + "mlp.w2.bias"].float().view(hid // 32, 32)], 1).reshape(2 * hid))
                 w[f"b{i}.fc2"], w[f"b{i}.fc2b"] = self._lin(P[p + "mlp.w3.weight"], tv), f32(P[p + "mlp.w3.bias"])
         w["norm.w"], w["norm.b"] = f32(P[Bk + "norm.weight"]), f32(P[Bk + "norm.bias"])
+        return w
+
+    def _pack_rest(self, P: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+        """The packed weights after the taps (SPM, extractors, adapter tail, FAPM, ups, decoder, seg head): the part that
+        differs between the folds of one training run."""
+        w = {}
+        A = "encoder.dinov3_adapter."
+        tr = self.tr
+        f32 = self._dev
         # ---- SPM
         S = A + "spm."
         w["stem0.w"] = f32(P[S + "stem.0.weight"])
@@ -245,9 +311,7 @@ class ForwardEngine:
                 w[f"d{s}.n{j}w"], w[f"d{s}.n{j}b"] = f32(P[p + "norm.weight"]), f32(P[p + "norm.bias"])
         w["seg.w"] = f32(P["decoder.seg_layers.2.weight"].reshape(self.ncls, -1))
         w["seg.b"] = f32(P["decoder.seg_layers.2.bias"])
-        self.w = w
-        self._plans.clear()
-        self._graphs.clear()
+        return w
 
     # ------------------------------------------------------------------ plan helpers
     def _rope_tables(self, h: int, wd: int) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -283,14 +347,18 @@ class ForwardEngine:
         plan.add(name, self.lib.b2u_gemm, C.byref(p))
 
     # ------------------------------------------------------------------ plan
-    def build_plan(self, B: int, S: int) -> Tuple[Plan, dict]:
+    def build_plan(self, B: int, S: int, w: Optional[Dict[str, torch.Tensor]] = None,
+                   share: Optional[Dict[str, torch.Tensor]] = None) -> Tuple[Plan, dict]:
+        """The (B, S) launch list on the weights `w` (default: the engine's own).  With `share` (the buffers of an
+        existing (B, S) plan) every activation buffer is taken from it instead of allocated."""
         if S < 128 or S % 128:
             # every pyramid level (S/2 ... S/32) must tile: conv row widths multiples of 4, the halo-mode convs multiples of 8,
             # the three-plane depthwise conv S/16 % 8 == 0 -> multiples of 128 (128, 256, 384, 512, 640, ...); the reference's
             # plans force 512
             raise ValueError("input size must be a multiple of 128 (the reference's plan forces 512x512); the fp32 tier takes "
                              "multiples of 32")
-        v, w, lib = self.v, self.w, self.lib
+        v, lib = self.v, self.lib
+        w = self.w if w is None else w
         vt, rt, tv, tr = self.vt, self.rt, self.tv, self.tr
         D, Hh = v.embed_dim, v.num_heads
         h = S // 16
@@ -303,8 +371,11 @@ class ForwardEngine:
         dev = self.device
         bufs: Dict[str, torch.Tensor] = {}
 
-        def buf(name, shape, dtype):
-            t = torch.empty(shape, dtype=dtype, device=dev)
+        def buf(name, shape, dtype, zero=False):
+            if share is not None:
+                t = share[name]
+            else:
+                t = (torch.zeros if zero else torch.empty)(shape, dtype=dtype, device=dev)
             bufs[name] = t
             return t
 
@@ -319,11 +390,11 @@ class ForwardEngine:
         hd = self.hd
         Q, K_ = buf("Q", (B, Hh, N, hd), tv), buf("K", (B, Hh, N, hd), tv)
         # V^T with zeroed padding columns (never written by the QKV epilogue)
-        V = bufs["V"] = torch.zeros((B, Hh, hd, npad), dtype=tv, device=dev)
+        V = buf("V", (B, Hh, hd, npad), tv, zero=True)
         O = buf("O", (T, D), tv)
         Hid = buf("Hid", (T, v.ffn_hidden), tv)
         taps = [buf(f"tap{k}", (B * P, D), torch.float32) for k in range(4)]
-        sin, cos = self._rope_tables(h, h)
+        sin, cos = (share["rope_sin"], share["rope_cos"]) if share is not None else self._rope_tables(h, h)
         bufs["rope_sin"], bufs["rope_cos"] = sin, cos
 
         plan.add("patchify", lib.b2u_patchify, _ptr(x), _ptr(Ape), B, S, vt)
@@ -477,7 +548,7 @@ class ForwardEngine:
         gate = buf("gate", (B, 256), torch.float32)
         wfl = max(int(lib.b2u_in_stats_work_floats(B, (S4 >> i) ** 2, oc)) for i, oc in enumerate(self.features))
         wfl = max([wfl] + [int(lib.b2u_in_stats_work_floats(B, (S4 << s) ** 2, self.features[2 - s])) for s in range(3)])
-        bufs["in_work"] = in_work = torch.zeros(wfl, dtype=torch.float32, device=dev)   # ticket counters start at zero
+        in_work = buf("in_work", (wfl,), torch.float32, zero=True)   # ticket counters start at zero
         feats = self.features
         cat = [buf("cat0", (B * S4 * S4, 2 * feats[2]), tr), buf("cat1", (B * S2 * S2, 2 * feats[1]), tr),
                buf("cat2", (B * S * S, 2 * feats[0]), tr)]
@@ -566,6 +637,7 @@ class ForwardEngine:
             return self._plans[key]
         while len(self._plans) >= max(1, self.max_plans):      # evict the least recently used buffer set + graph
             old, _ = self._plans.popitem(last=False)
+            self._fold_plans.pop(old, None)
             for gk in [k for k in self._graphs if k[:2] == old]:
                 self._graphs.pop(gk)
         with torch.cuda.device(self.device):                   # kernels, TMA maps and num_sms() use the current device
@@ -580,6 +652,61 @@ class ForwardEngine:
         """Frees every cached (batch, size) buffer set and CUDA graph."""
         self._plans.clear()
         self._graphs.clear()
+        self._fold_plans.clear()
+
+    # ------------------------------------------------------------------ fold ensembles on one backbone
+    def pack_folds(self, fold_params: Iterable[Dict[str, torch.Tensor]]):
+        """Packs the weights after the taps of every fold (reference-keyed state dicts whose backbone is the one this
+        engine was packed with: the backbone is frozen in training, so every fold of a run has it bit for bit).  The
+        ViT section stays packed once; each fold adds only its trainable weights, and its "rest" launch list runs on the
+        activation, tap and input buffers of the shared (B, S) plan."""
+        with torch.cuda.device(self.device):
+            folds = [self._pack_rest(P) for P in fold_params]
+        self._folds = folds
+        self._fold_plans.clear()
+        for gk in [k for k in self._graphs if len(k) == 4 and k[2] == "fold"]:
+            self._graphs.pop(gk)
+
+    @property
+    def num_folds(self) -> int:
+        return len(self._folds)
+
+    def fold_bytes(self) -> List[int]:
+        """Device bytes of each fold's packed weights."""
+        return [sum(t.numel() * t.element_size() for t in f.values() if t.is_cuda) for f in self._folds]
+
+    def _fold_plan(self, B: int, S: int, f: int) -> Plan:
+        _, bufs = self.get_plan(B, S)
+        plans = self._fold_plans.setdefault((B, S), [None] * len(self._folds))
+        if plans[f] is None:
+            w = dict(self.w)
+            w.update(self._folds[f])
+            with torch.cuda.device(self.device):
+                if self.precision == "fp32":
+                    from .engine_fp32 import build_plan_fp32
+                    plans[f], _ = build_plan_fp32(self, B, S, w=w, share=bufs)
+                else:
+                    plans[f], _ = self.build_plan(B, S, w=w, share=bufs)
+        return plans[f]
+
+    def run_fold_rest(self, B: int, S: int, f: int, use_graph: bool = False) -> Tuple[torch.Tensor, torch.Tensor]:
+        """`run_resident(B, S, part="rest")` on fold f's weights (`pack_folds`): SPM .. seg head on whatever the shared
+        plan's input and tap buffers hold, into its logits / labels buffers (overwritten by the next fold)."""
+        if not 0 <= f < len(self._folds):
+            raise IndexError(f"fold {f} of {len(self._folds)} packed fold weight sets")
+        plan = self._fold_plan(B, S, f)
+        _, bufs = self.get_plan(B, S)
+        with torch.cuda.device(self.device):
+            stream = torch.cuda.current_stream(self.device).cuda_stream
+            if use_graph:
+                key = (B, S, "fold", f)
+                g = self._graphs.get(key)
+                if g is None:
+                    g = self._graphs[key] = self._capture(plan, stream, plan.vit_end, None)
+                g.replay()
+            else:
+                plan.run(stream, plan.vit_end)
+        return bufs["logits"], bufs["labels"]
 
     def forward(self, x: torch.Tensor, use_graph: bool = False) -> Tuple[torch.Tensor, torch.Tensor]:
         """x: fp32 [B, 3, S, S] on the engine's device -> (logits fp32 [B, ncls, S, S], labels uint8 [B, S, S]).
@@ -595,6 +722,16 @@ class ForwardEngine:
         bufs["x"].copy_(x, non_blocking=True)
         return self.run_resident(B, S, use_graph)
 
+    def _capture(self, plan: Plan, stream: int, lo: int, hi: Optional[int]):
+        """calls[lo:hi] of `plan` as a CUDA graph, with no other thread's device work in flight (`GRAPH_CAPTURE`)."""
+        with GRAPH_CAPTURE.capture():
+            plan.run(stream, lo, hi)  # warm-up (cudaFuncSetAttribute etc. must happen outside capture)
+            torch.cuda.synchronize(self.device)
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                plan.run(torch.cuda.current_stream(self.device).cuda_stream, lo, hi)
+        return g
+
     def run_resident(self, B: int, S: int, use_graph: bool = False, part: str = "all") -> Tuple[torch.Tensor, torch.Tensor]:
         """Runs the (B, S) plan on whatever `get_plan(B, S)[1]["x"]` holds (a producer kernel, e.g. the sliding-window
         tile gather, wrote the batch there on the current stream).  part: "all", "vit" (patch embed .. ViT taps only) or
@@ -607,12 +744,7 @@ class ForwardEngine:
                 key = (B, S, part)
                 g = self._graphs.get(key)
                 if g is None:
-                    plan.run(stream, lo, hi)  # warm-up (cudaFuncSetAttribute etc. must happen outside capture)
-                    torch.cuda.synchronize(self.device)
-                    g = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(g):
-                        plan.run(torch.cuda.current_stream(self.device).cuda_stream, lo, hi)
-                    self._graphs[key] = g
+                    g = self._graphs[key] = self._capture(plan, stream, lo, hi)
                 g.replay()
             else:
                 plan.run(stream, lo, hi)

@@ -26,11 +26,14 @@ def _patch_attention_rope(args, sin: int, cos: int, keep: list):
     return (args[0], sin, cos) + tuple(args[3:])
 
 
-def build_plan_fp32(eng, B: int, S: int):
+def build_plan_fp32(eng, B: int, S: int, w=None, share=None):
+    """The (B, S) launch list of the fp32 tier on the weights `w` (default: the engine's own); with `share` (the buffers
+    of an existing (B, S) plan) every buffer is taken from it instead of allocated."""
     from .engine import Plan
     if S % 32 or S < 64:
         raise ValueError("fp32 tier: input size must be a multiple of 32 (>= 64)")
-    v, w, lib = eng.v, eng.w, eng.lib
+    v, lib = eng.v, eng.lib
+    w = eng.w if w is None else w
     if v.ffn_layer != "mlp":
         raise NotImplementedError("fp32 parity tier implements the Mlp FFN variants (dinounet_s/b/l); SwiGLU (7B) runs on the "
                                   "16-bit tensor-core path only")
@@ -47,7 +50,7 @@ def build_plan_fp32(eng, B: int, S: int):
     bufs: Dict[str, torch.Tensor] = {}
 
     def buf(name, shape, dtype=f32):
-        t = torch.empty(shape, dtype=dtype, device=dev)
+        t = share[name] if share is not None else torch.empty(shape, dtype=dtype, device=dev)
         bufs[name] = t
         return t
 
@@ -88,7 +91,7 @@ def build_plan_fp32(eng, B: int, S: int):
     O = buf("O", (T, D))
     Hid = buf("Hid", (T, v.ffn_hidden))
     taps = [buf(f"tap{k}", (B * P, D)) for k in range(4)]
-    sin, cos = eng._rope_tables(h, h)
+    sin, cos = (share["rope_sin"], share["rope_cos"]) if share is not None else eng._rope_tables(h, h)
     bufs["rope_sin"], bufs["rope_cos"] = sin, cos
     plan.add("patchify", lib.b2u_f32_patchify, _ptr(x), _ptr(Ape), B, S)
     gemm("patch_embed", Ape, B * P, 768, 768, w["pe.w"], D, X, D, bias=w["pe.b"], rows=(P, N, cfg.N_PREFIX))

@@ -471,12 +471,19 @@ class UNetDecoder(_NoForward):
 
 
 # ----------------------------------------------------------------------------------------------- DinoUNet
+#: `dinov3_pretrained_path` of a network whose weights, backbone included, come from a training checkpoint next: the
+#: backbone is built without reading a pretrained file
+BACKBONE_FROM_CHECKPOINT = object()
+
+
 def load_dinov3_model(model_name: str, pretrained_path: str = None) -> DinoVisionTransformer:
     """dinounet_training.py:51-75.  The reference downloads weights when the path is missing; this box has no network,
     so that branch raises unless DINOUNET_B200_ALLOW_RANDOM_BACKBONE=1 (random-init backbone: benchmarks / tests)."""
     if model_name not in cfg.VARIANTS:
         raise ValueError(f"Unsupported model: {model_name}. Supported models: {list(cfg.VARIANTS)}")
     model = make_backbone(model_name)
+    if pretrained_path is BACKBONE_FROM_CHECKPOINT:
+        return model
     if pretrained_path and os.path.exists(pretrained_path):
         state_dict = torch.load(pretrained_path, map_location="cpu")
         model.load_state_dict(state_dict, strict=True)
@@ -565,6 +572,8 @@ class DinoUNet(nn.Module):
                                    nonlin_first=nonlin_first)
         self._engine = None
         self._repack_before_eval = False
+        #: advances whenever the weights may have changed (a state dict loaded, `repack()`, a move / cast)
+        self.weights_version = 0
         self.register_load_state_dict_post_hook(lambda module, incompatible: module._invalidate())
 
     def _create_dinov3_encoder(self, pretrained_path, model_name, features_per_stage, conv_op, norm_op, norm_op_kwargs,
@@ -586,14 +595,15 @@ class DinoUNet(nn.Module):
     # ---- engine management -------------------------------------------------------------------------------------
     def _invalidate(self):
         self._engine = None
+        self.weights_version = getattr(self, "weights_version", 0) + 1
 
     def _apply(self, fn, *a, **k):
-        self._engine = None
+        self._invalidate()
         return super()._apply(fn, *a, **k)
 
     def repack(self):
         """Call after mutating parameters in place (e.g. an optimizer step) to refresh the packed kernel weights."""
-        self._engine = None
+        self._invalidate()
 
     def _eval_engine(self, device):
         """The engine for eval-path entries.  A "reference"-semantics train forward changes the BatchNorm running statistics
@@ -634,14 +644,19 @@ class DinoUNet(nn.Module):
                                       "unsupported plan entries: " + "; ".join(bad))
 
     def _get_engine(self, device):
-        from ..engine import ForwardEngine
         if self._engine is None or self._engine.device != device:
-            self._check_block_spec()
-            sd = {k: t for k, t in self.state_dict().items() if not k.startswith("decoder.encoder.")}
-            self._engine = ForwardEngine(self.dinov3_model_name, sd, self.num_classes, device, self.vit_dtype,
-                                         self.rest_dtype, tuple(self.encoder.target_channels), self.attn_impl,
-                                         getattr(self, "query_dtype", "fp32"), getattr(self, "precision", "16"))
+            self._engine = self.new_engine(self.state_dict(), device)
         return self._engine
+
+    def new_engine(self, state_dict, device):
+        """A forward engine with this network's settings on the weights of `state_dict` (reference keys), separate from
+        the network's own."""
+        from ..engine import ForwardEngine
+        self._check_block_spec()
+        sd = {k: t for k, t in state_dict.items() if not k.startswith("decoder.encoder.")}
+        return ForwardEngine(self.dinov3_model_name, sd, self.num_classes, device, self.vit_dtype, self.rest_dtype,
+                             tuple(self.encoder.target_channels), self.attn_impl, getattr(self, "query_dtype", "fp32"),
+                             getattr(self, "precision", "16"))
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         if self.decoder.deep_supervision:

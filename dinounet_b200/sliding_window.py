@@ -14,6 +14,7 @@ averaged, gaussian-weighted and accumulated by one small kernel.  Nothing crosse
 volume and the download of the result.
 """
 import itertools
+import math
 from types import SimpleNamespace
 from typing import List, Optional, Sequence, Tuple
 
@@ -73,6 +74,34 @@ def compute_gaussian(tile_size: Sequence[int], sigma_scale: float = 1. / 8, valu
     return g
 
 
+def backbones_identical(list_of_parameters) -> bool:
+    """True when there are at least two state dicts and every one holds the same DINOv3 backbone, bit for bit: the
+    `*.dinov3_adapter.backbone.*` tensors, the `decoder.encoder.` duplicates included.  Training freezes the backbone,
+    so the folds of one run pass this."""
+    if not list_of_parameters or len(list_of_parameters) < 2:
+        return False
+
+    def backbone(sd):
+        return {k: t for k, t in sd.items() if ".dinov3_adapter.backbone." in k}
+
+    first = backbone(list_of_parameters[0])
+    if not first:
+        return False
+    for sd in list_of_parameters[1:]:
+        other = backbone(sd)
+        if other.keys() != first.keys():
+            return False
+        for k, a in first.items():
+            b = other[k]
+            if a.dtype != b.dtype or a.shape != b.shape:
+                return False
+            a8 = a.detach().contiguous().reshape(-1).view(torch.uint8)
+            b8 = b.detach().to(a.device).contiguous().reshape(-1).view(torch.uint8)
+            if not torch.equal(a8, b8):
+                return False
+    return True
+
+
 def pad_to_patch_size(image: torch.Tensor, patch_size: Sequence[int]):
     """What the reference obtains from acvl_utils' `pad_nd_image(image, patch_size, 'constant', {'value': 0}, True)`
     (predict_from_raw_data.py:703-705): zero-pad the trailing dims, centred, up to the patch size; plus the slicer
@@ -109,6 +138,14 @@ class SlidingWindowPredictor:
         self.perform_everything_on_device = perform_everything_on_device
         self.tile_batch = int(tile_batch)
         self.use_graph = use_graph
+        #: slices per chunk of the shared-backbone fold route; None = the fewest slices that fill whole tile batches,
+        #: times the multiple that makes about four batches
+        self.fold_chunk_slices = None
+        #: the fold ensemble route the last `predict_logits_from_preprocessed_data` took: "shared_backbone" (one ViT
+        #: pass per tile batch for every fold) or "per_fold" (the weights reloaded for each fold)
+        self.ensemble_route = None
+        self._shared_backbone_params = None
+        self._fold_engine = None
 
     def manual_initialization(self, network, plans_manager, configuration_manager, parameters: Optional[List[dict]],
                               dataset_json: dict, trainer_name: str,
@@ -126,6 +163,56 @@ class SlidingWindowPredictor:
             self.label_manager = plans_manager.get_label_manager(dataset_json)
         else:
             self.label_manager = SimpleNamespace(num_segmentation_heads=network.num_classes)
+        self._select_ensemble_route()
+
+    def _select_ensemble_route(self):
+        """Folds that share the backbone bit for bit run it once per tile batch; decided once, for this
+        `list_of_parameters` (a list assigned later takes the per-fold route)."""
+        params = self.list_of_parameters
+        self._shared_backbone_params = params if backbones_identical(params) else None
+        self._fold_engine = None
+
+    def initialize_from_trained_model_folder(self, model_training_output_dir: str, use_folds,
+                                             checkpoint_name: str = "checkpoint_final.pth"):
+        """predict_from_raw_data.py:67-130: plans, dataset.json and the fold checkpoints of a trained model folder
+        (use_folds None = every `fold_<k>` with the checkpoint, "all" = `fold_all`).  The trainer name, configuration and
+        mirroring axes come from the first checkpoint; the network is the native `DinoUNet` of that trainer's variant,
+        built on the device with the first fold's weights.  Folds that share the backbone (the folds of one run) run it
+        once per tile batch."""
+        from . import predict as PR
+        from .checkpoint import match_keys
+        pm, cm, dj, parameters, trainer_name, _, mirror_axes = PR.load_model_folder(
+            model_training_output_dir, use_folds, checkpoint_name)
+        heads = pm.get_label_manager(dj).num_segmentation_heads
+        network = PR.build_network(trainer_name, cm, PR.num_input_channels(dj), heads)
+        own = set(network.state_dict().keys())
+        parameters = [match_keys(p, own) for p in parameters]
+        network.load_state_dict(parameters[0])
+        self.manual_initialization(network.to(self.device), pm, cm, parameters, dj, trainer_name, mirror_axes)
+
+    def predict_from_files(self, list_of_lists_or_source_folder, output_folder_or_list_of_truncated_output_files,
+                           save_probabilities: bool = False, overwrite: bool = True, num_processes_preprocessing: int = 3,
+                           num_processes_segmentation_export: int = 3, folder_with_segs_from_prev_stage: str = None,
+                           num_parts: int = 1, part_id: int = 0):
+        """predict_from_raw_data.py:207-266 on the device (see dinounet_b200/predict.py): cases `<id>_<4 digits>` of a
+        folder, or lists of files, to `<output>/<id><file_ending>` (and `.npz` / `.pkl` with `save_probabilities`),
+        this part's share `[part_id::num_parts]`, finished cases skipped when `overwrite` is False."""
+        from . import predict as PR
+        return PR.predict_from_files(self, list_of_lists_or_source_folder, output_folder_or_list_of_truncated_output_files,
+                                     save_probabilities, overwrite, num_processes_preprocessing,
+                                     num_processes_segmentation_export, folder_with_segs_from_prev_stage, num_parts,
+                                     part_id)
+
+    def predict_from_list_of_npy_arrays(self, image_or_list_of_images, segs_from_prev_stage_or_list_of_segs_from_prev_stage,
+                                        properties_or_list_of_properties, truncated_ofname, num_processes: int = 3,
+                                        save_probabilities: bool = False, num_processes_segmentation_export: int = 3):
+        """predict_from_raw_data.py:343-359 on the device: images [C, X, Y, Z] with their properties ('spacing') to the
+        truncated output names, or, where there is none, the segmentation (and probabilities) returned."""
+        from . import predict as PR
+        return PR.predict_from_list_of_npy_arrays(self, image_or_list_of_images,
+                                                  segs_from_prev_stage_or_list_of_segs_from_prev_stage,
+                                                  properties_or_list_of_properties, truncated_ofname, num_processes,
+                                                  save_probabilities, num_processes_segmentation_export)
 
     def initialize_from_checkpoint(self, network, filename_or_checkpoint, patch_size=(512, 512)):
         """Weights + mirroring axes from a training checkpoint (`checkpoint_final.pth`), the part of
@@ -231,6 +318,10 @@ class SlidingWindowPredictor:
         from .preprocess import ensemble_logits
         lib = L.load()
         params = self.list_of_parameters
+        if params and params is self._shared_backbone_params:
+            self.ensemble_route = "shared_backbone"
+            return self._predict_folds_shared_backbone(data)
+        self.ensemble_route = "per_fold"
 
         def runs():
             for p in (params or [None]):
@@ -248,6 +339,126 @@ class SlidingWindowPredictor:
                         "b2u_pre_ensemble_f16")
 
         return ensemble_logits(runs(), len(params) if params else 1, add)
+
+    def _shared_fold_engine(self, dev: torch.device):
+        """An engine of its own with the shared backbone packed once and every fold's weights after the taps, kept
+        across calls for this `list_of_parameters` while the network's weights stay as this method left them.  It
+        loads the last fold into the network (so the network holds it, as after the per-fold route) and packs the
+        backbone from the network's own parameters, as the network's engine does."""
+        params = self.list_of_parameters
+        net = self.network
+        cached = self._fold_engine
+        if (cached is not None and cached[0] is params and cached[1] is net and cached[2] == net.weights_version
+                and not net._repack_before_eval and cached[3].device == dev):
+            return cached[3]
+        self._fold_engine = None
+        net.load_state_dict(params[-1])
+        net._repack_before_eval = False     # the load already dropped the network's packed weights
+
+        # the folds are packed from device copies of their weights after the taps, one fold at a time: BatchNorm folded
+        # on the host rounds differently in the last bit from the network's engine, which packs device tensors
+        def after_taps_on_device(sd):
+            return {k: t.to(dev) for k, t in sd.items() if ".dinov3_adapter.backbone." not in k}
+
+        eng = net.new_engine(net.state_dict(), dev)
+        eng.pack_folds(after_taps_on_device(p) for p in params)
+        self._fold_engine = (params, net, net.weights_version, eng)
+        return eng
+
+    def _fold_chunk(self, tiles_per_slice: int, D: int) -> int:
+        if self.fold_chunk_slices is not None:
+            return max(1, min(int(self.fold_chunk_slices), D))
+        per = max(1, self.tile_batch)
+        k0 = per // math.gcd(per, tiles_per_slice)     # slices whose tiles fill whole batches
+        return max(1, min(k0 * max(1, (4 * per) // (k0 * tiles_per_slice)), D))
+
+    @torch.no_grad()
+    def _predict_folds_shared_backbone(self, input_image: torch.Tensor) -> torch.Tensor:
+        """The fold ensemble when every fold holds the same backbone.  Per tile batch: one gather, one ViT pass, then
+        each fold's SPM .. seg head on the shared taps, its logits accumulated before the next fold overwrites them.
+        2-D tiles never mix slices, so the case runs in chunks of slices: each fold's fp16 accumulator covers one chunk,
+        the gaussian weight count (the same for every fold) is kept once, and after the chunk each fold is finalized and
+        the folds are combined in the order of `ensemble_logits`.  Every voxel sees the operations of the per-fold route,
+        so the result has its bits.  Afterwards the network holds the last fold's weights, as after the per-fold route."""
+        assert isinstance(input_image, torch.Tensor)
+        assert input_image.ndim == 4, "input_image must be a 4D np.ndarray or torch.Tensor (c, x, y, z)"
+        params = self.list_of_parameters
+        net = self.network
+        net.eval()
+        patch = [int(p) for p in self.configuration_manager.patch_size]
+        if len(patch) != 2 or patch[0] != patch[1]:
+            raise NotImplementedError("the native engine runs square 2D patches (main_dinov3 forces 512x512)")
+        lib = L.load()
+        dev = self.device if self.device.index is not None else torch.device("cuda", torch.cuda.current_device())
+        heads = int(self.label_manager.num_segmentation_heads)
+        nf = len(params)
+        data, revert = pad_to_patch_size(input_image, patch)
+        slicers = self._internal_get_sliding_window_slicers(tuple(data.shape[1:]))
+        data = data.to(dev, dtype=torch.float32, non_blocking=True).contiguous()
+        Cin, D, H, W = data.shape
+        th = tw = patch[0]
+        variants = self._mirror_variants()
+        nvar = len(variants)
+        tiles = [(s[1], s[2].start, s[3].start) for s in slicers]
+        tps = len(tiles) // D
+        per = max(1, self.tile_batch)
+        nb = per * nvar
+        chunk = self._fold_chunk(tps, D)
+        gaussian = compute_gaussian(tuple(patch), sigma_scale=1. / 8, value_scaling_factor=10,
+                                    device=dev) if self.use_gaussian else None
+        eng = self._shared_fold_engine(dev)
+        if eng.ncls != heads:
+            raise ValueError(f"network produces {eng.ncls} heads, label manager expects {heads}")
+        _, bufs = eng.get_plan(nb, th)
+        hs, ws = revert[2], revert[3]
+        out = torch.empty((heads, D, hs.stop - hs.start, ws.stop - ws.start), dtype=torch.half, device=dev)
+        acc_all = torch.empty(nf * heads * chunk * H * W, dtype=torch.half, device=dev)
+        npred_all = torch.empty(chunk * H * W, dtype=torch.half, device=dev)
+        flag = torch.zeros(1, dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            for d0 in range(0, D, chunk):
+                dc = min(chunk, D - d0)
+                plane = dc * H * W
+                ctiles = tiles[d0 * tps:(d0 + dc) * tps]
+                n_batches = (len(ctiles) + per - 1) // per
+                desc = np.zeros((n_batches, nb, 4), dtype=np.int32)
+                for t, (d, y0, x0) in enumerate(ctiles):        # slices relative to the chunk
+                    for v, bits in enumerate(variants):
+                        desc[t // per, (t % per) * nvar + v] = (d - d0, y0, x0, bits)
+                for t in range(len(ctiles), n_batches * per):   # fill the last batch with repeats of the chunk's first tile
+                    desc[t // per, (t % per) * nvar:(t % per + 1) * nvar] = desc[0, :nvar]
+                desc_dev = torch.from_numpy(desc).to(dev)
+                accs = [acc_all[f * heads * plane:(f + 1) * heads * plane].view(heads, dc, H, W) for f in range(nf)]
+                acc_all[:nf * heads * plane].zero_()
+                npred = npred_all[:plane].zero_()
+                vol = data.data_ptr() + d0 * H * W * data.element_size()   # slice d0 of channel 0; channel stride D*H*W
+                for b in range(n_batches):
+                    dptr = desc_dev[b].data_ptr()
+                    L.check(lib.b2u_sw_gather_tiles(vol, bufs["x"].data_ptr(), dptr, nb, Cin, D, H, W, th, tw, stream),
+                            "sw_gather_tiles")
+                    eng.run_resident(nb, th, self.use_graph, part="vit")
+                    for f in range(nf):
+                        logits, _ = eng.run_fold_rest(nb, th, f, self.use_graph)
+                        for t in range(min(per, len(ctiles) - b * per)):
+                            L.check(lib.b2u_sw_accumulate(logits.data_ptr(), dptr, t * nvar, nvar,
+                                                          gaussian.data_ptr() if gaussian is not None else None,
+                                                          accs[f].data_ptr(), npred.data_ptr() if f == 0 else None,
+                                                          heads, dc, H, W, th, tw, stream), "sw_accumulate")
+                for f in range(nf):
+                    L.check(lib.b2u_sw_finalize(accs[f].data_ptr(), npred.data_ptr(), heads, plane, flag.data_ptr(),
+                                                stream), "sw_finalize")
+                for f in range(1, nf):
+                    L.check(lib.b2u_pre_ensemble_f16(accs[0].data_ptr(), accs[f].data_ptr(), heads * plane, 0, stream),
+                            "b2u_pre_ensemble_f16")
+                L.check(lib.b2u_pre_ensemble_f16(accs[0].data_ptr(), None, heads * plane, nf, stream),
+                        "b2u_pre_ensemble_f16")
+                out[:, d0:d0 + dc].copy_(accs[0][:, :, hs, ws])
+        if int(flag.item()):
+            raise RuntimeError("Encountered inf in predicted array. Aborting... If this problem persists, "
+                               "reduce value_scaling_factor in compute_gaussian or increase the dtype of "
+                               "predicted_logits to fp32")
+        return out
 
     def predict_single_npy_array(self, input_image: np.ndarray, image_properties: dict,
                                  segmentation_previous_stage: np.ndarray = None, output_file_truncated: str = None,

@@ -181,6 +181,7 @@ class DinoUNetTrainer(_Base):
         `validation/summary.json`.  The cascade and next-stage predictions are not implemented: they raise before
         anything runs."""
         from . import evaluation, export
+        from .engine import GRAPH_CAPTURE
         from .sliding_window import SlidingWindowPredictor
         if self.is_cascaded:
             raise NotImplementedError("the final validation on the device does not implement the cascade")
@@ -203,7 +204,7 @@ class DinoUNetTrainer(_Base):
         stream = torch.cuda.current_stream(predictor.device if predictor.device.index is not None else None)
 
         def write(logits, properties, output_filename_truncated):
-            with torch.cuda.stream(stream):
+            with GRAPH_CAPTURE.device_work(), torch.cuda.stream(stream):
                 export.export_prediction_from_logits(logits, properties, self.configuration_manager, self.plans_manager,
                                                      self.dataset_json, output_filename_truncated, save_probabilities)
 

@@ -198,7 +198,8 @@ int b2u_msda_backward_f32(const float* value, const int64_t* spatial_shapes, con
  * b2u_sw_accumulate: one tile whose mirror variants are logits[first .. first+nvar) (fp32 [n, C, th, tw], variant 0
  *   unflipped, nvar in {1,2,4}): un-mirror, mean over variants, * gaussian (fp16 [th, tw], NULL = 1), accumulate into
  *   acc fp16 [C, D, H, W] and npred fp16 [D, H, W] with the reference's fp16 rounding sequence (:545-551, :598-599).
- *   Launches for overlapping tiles must be stream-ordered.
+ *   npred NULL: accumulate into acc only (the folds of an ensemble share one gaussian weight count, which one call per
+ *   tile adds).  Launches for overlapping tiles must be stream-ordered.
  * b2u_sw_finalize: acc /= npred (:601); *inf_flag |= 1 if any result is inf (:603-606 raises). */
 int b2u_sw_gather_tiles(const float* volume, float* batch, const int32_t* tile_desc, int32_t n_entries, int32_t Cin,
                         int32_t D, int32_t H, int32_t W, int32_t th, int32_t tw, b2u_stream_t stream);
