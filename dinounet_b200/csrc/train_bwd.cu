@@ -85,7 +85,10 @@ extern "C" int b2u_f32_colsum(const float* in, int64_t ld, int64_t rows, int32_t
 }
 
 // ---------------------------------------------------------------------------------------- LayerNorm backward
-// one warp per row (grid-stride); dx = rstd * (g - mean(g) - xhat * mean(g * xhat)), g = dy * w;  dw += dy * xhat, db += dy
+// one warp per row (grid-stride); dx = rstd * (g - mean(g) - xhat * mean(g * xhat)), g = dy * w;  dw += dy * xhat, db += dy.
+// blockIdx.y picks a chunk of LN_BWD_COLS columns: the row statistics cover the whole row, dx and the dw / db partials
+// this chunk only (one chunk up to D = 1024, four at dinounet_7b's 4096)
+constexpr int LN_BWD_COLS = 1024;
 __global__ void __launch_bounds__(256) f32_layernorm_bwd_kernel(const float* __restrict__ x, const float* __restrict__ w,
                                                                 const float* __restrict__ dy, float* __restrict__ dx,
                                                                 float* __restrict__ dw, float* __restrict__ db, long long rows,
@@ -93,7 +96,8 @@ __global__ void __launch_bounds__(256) f32_layernorm_bwd_kernel(const float* __r
   const int lane = threadIdx.x & 31;
   const long long warp0 = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   const long long nwarps = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
-  float pw[32], pb[32];                       // column partials of this lane: columns lane + 32 i  (D <= 1024)
+  const int c0 = blockIdx.y * LN_BWD_COLS, c1 = min(D, c0 + LN_BWD_COLS);
+  float pw[32], pb[32];                       // column partials of this lane: columns c0 + lane + 32 i
 #pragma unroll
   for (int i = 0; i < 32; ++i) { pw[i] = 0.f; pb[i] = 0.f; }
   for (long long r = warp0; r < rows; r += nwarps) {
@@ -110,13 +114,16 @@ __global__ void __launch_bounds__(256) f32_layernorm_bwd_kernel(const float* __r
     for (int o = 16; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
     const float rstd = 1.0f / sqrtf(q / D + eps);
     float m1 = 0.f, m2 = 0.f;
+    for (int c = lane; c < D; c += 32) {
+      const float xh = (xr[c] - mean) * rstd, g = gr[c] * w[c];
+      m1 += g;
+      m2 = fmaf(g, xh, m2);
+    }
 #pragma unroll
     for (int i = 0; i < 32; ++i) {
-      const int c = lane + 32 * i;
-      if (c < D) {
-        const float xh = (xr[c] - mean) * rstd, g = gr[c] * w[c];
-        m1 += g;
-        m2 = fmaf(g, xh, m2);
+      const int c = c0 + lane + 32 * i;
+      if (c < c1) {
+        const float xh = (xr[c] - mean) * rstd;
         pw[i] = fmaf(gr[c], xh, pw[i]);
         pb[i] += gr[c];
       }
@@ -124,23 +131,24 @@ __global__ void __launch_bounds__(256) f32_layernorm_bwd_kernel(const float* __r
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) { m1 += __shfl_xor_sync(0xffffffffu, m1, o); m2 += __shfl_xor_sync(0xffffffffu, m2, o); }
     m1 /= D; m2 /= D;
-    for (int c = lane; c < D; c += 32) {
+    for (int c = c0 + lane; c < c1; c += 32) {
       const float xh = (xr[c] - mean) * rstd;
       dx[r * D + c] = rstd * (gr[c] * w[c] - m1 - xh * m2);
     }
   }
 #pragma unroll
   for (int i = 0; i < 32; ++i) {
-    const int c = lane + 32 * i;
-    if (c < D) { atomicAdd(&dw[c], pw[i]); atomicAdd(&db[c], pb[i]); }
+    const int c = c0 + lane + 32 * i;
+    if (c < c1) { atomicAdd(&dw[c], pw[i]); atomicAdd(&db[c], pb[i]); }
   }
 }
 extern "C" int b2u_f32_layernorm_bwd(const float* x, const float* w, const float* dy, float* dx, float* dw, float* db,
                                      int64_t rows, int32_t D, float eps, b2u_stream_t s) {
-  if (D > 1024) return set_error(-1, "b2u_f32_layernorm_bwd: D <= 1024");
+  if (D < 1) return set_error(-1, "b2u_f32_layernorm_bwd: D %d", D);
   const long long want = (rows + 7) / 8;
   const unsigned grid = static_cast<unsigned>(want < 1184 ? (want < 1 ? 1 : want) : 1184);
-  f32_layernorm_bwd_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(s)>>>(x, w, dy, dx, dw, db, rows, D, eps);
+  const dim3 g(grid, (D + LN_BWD_COLS - 1) / LN_BWD_COLS);
+  f32_layernorm_bwd_kernel<<<g, 256, 0, static_cast<cudaStream_t>(s)>>>(x, w, dy, dx, dw, db, rows, D, eps);
   return check_launch("f32_layernorm_bwd");
 }
 

@@ -517,6 +517,10 @@ class DinoUNet(nn.Module):
     #: num_batches_tracked (all-reduced across the ranks of the default process group), DropPath(0.3) on the extractors'
     #: ConvFFN branch and a log-uniform RoPE coordinate factor in [1/2, 2] per ViT block (see `train_forward`)
     train_semantics = "oracle"
+    #: True = the training step keeps only each adapter extractor's input query and recomputes the extractor in the
+    #: backward, as the reference's `with_cp=True` does (less activation memory, one more extractor forward per step);
+    #: the logits and gradients are those of False
+    train_recompute = False
 
     def __init__(self, network_config: dict = None, input_channels: int = None, num_classes: int = None,
                  dinov3_pretrained_path: str = "dinounet/checkpoints/dinov3_vits16_pretrain_lvd1689m-08c60483.pth",
@@ -717,6 +721,9 @@ class DinoUNet(nn.Module):
         sem = self.train_semantics
         if sem not in ("oracle", "reference"):
             raise ValueError(f"train_semantics must be 'oracle' or 'reference', got {sem!r}")
+        recompute = self.train_recompute
+        if not isinstance(recompute, bool):
+            raise ValueError(f"train_recompute must be True or False, got {recompute!r}")
         if sem == "reference":
             if self.dinov3_model_name.startswith("dinounet_7b"):
                 raise NotImplementedError("train_semantics='reference' does not cover dinounet_7b: its ViT's train-mode "
@@ -731,7 +738,7 @@ class DinoUNet(nn.Module):
             with torch.no_grad():
                 taps = self._get_engine(x.device).extract_vit_features(x)
             P = self.state_dict(keep_vars=True)
-            return trainable_forward(P, self.dinov3_model_name, x, taps, self.num_classes, gemm)
+            return trainable_forward(P, self.dinov3_model_name, x, taps, self.num_classes, gemm, recompute=recompute)
         B = x.shape[0]
         depth = cfg.VARIANTS[self.dinov3_model_name].depth
         with torch.no_grad():
@@ -748,7 +755,7 @@ class DinoUNet(nn.Module):
         P = self.state_dict(keep_vars=True)
         mode = TrainMode(bn=bn, drop_scale=(drop_keep / self._DROP_KEEP).contiguous(), sync=_bn_sync())
         self._repack_before_eval = True
-        return trainable_forward(P, self.dinov3_model_name, x, taps, self.num_classes, gemm, mode)
+        return trainable_forward(P, self.dinov3_model_name, x, taps, self.num_classes, gemm, mode, recompute)
 
     @torch.no_grad()
     def predict_labels(self, x: torch.Tensor) -> torch.Tensor:

@@ -24,12 +24,14 @@ Layout: activations are 2-D fp32 tensors [rows, C] (tokens, or NHWC pixels), exa
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Tuple
 
 import torch
 from torch.autograd import Function
+from torch.utils.checkpoint import checkpoint
 
 from . import config as cfg
 from . import lib as L
@@ -516,24 +518,59 @@ class TrainMode:
     sync: bool = False
 
 
-def trainable_forward(P: Dict[str, torch.Tensor], variant: str, x: torch.Tensor, taps: List[torch.Tensor], num_classes: int,
-                      gemm: str = "tf32", train_mode: Optional[TrainMode] = None) -> torch.Tensor:
-    """Differentiable forward of everything outside the frozen backbone.  P: reference-keyed parameters / buffers
-    (`net.state_dict(keep_vars=True)`), x [B,3,S,S] fp32, taps: 4 x [B, P, D] fp32 (frozen ViT outputs) -> logits [B,C,S,S].
-    gemm: matrix-product tier, "tf32" (tensor cores) or "fp32" (SIMT parity tier); the backward uses the same tier.
-    train_mode: None = eval-mode modules (BatchNorm on running statistics, DropPath off); a TrainMode = batch-statistics
-    BatchNorm that updates the running statistics in P, and DropPath with the given factors."""
+@contextlib.contextmanager
+def _gemm_tier(tier: str):
     global _GEMM_TIER
-    if gemm not in ("tf32", "fp32"):
-        raise ValueError(f"gemm tier must be 'tf32' or 'fp32', got {gemm!r}")
-    prev, _GEMM_TIER = _GEMM_TIER, gemm
+    prev, _GEMM_TIER = _GEMM_TIER, tier
     try:
-        return _trainable_forward(P, variant, x, taps, num_classes, train_mode)
+        yield
     finally:
         _GEMM_TIER = prev
 
 
-def _trainable_forward(P, variant, x, taps, num_classes, train_mode=None):
+def trainable_forward(P: Dict[str, torch.Tensor], variant: str, x: torch.Tensor, taps: List[torch.Tensor], num_classes: int,
+                      gemm: str = "tf32", train_mode: Optional[TrainMode] = None, recompute: bool = False) -> torch.Tensor:
+    """Differentiable forward of everything outside the frozen backbone.  P: reference-keyed parameters / buffers
+    (`net.state_dict(keep_vars=True)`), x [B,3,S,S] fp32, taps: 4 x [B, P, D] fp32 (frozen ViT outputs) -> logits [B,C,S,S].
+    gemm: matrix-product tier, "tf32" (tensor cores) or "fp32" (SIMT parity tier); the backward uses the same tier.
+    train_mode: None = eval-mode modules (BatchNorm on running statistics, DropPath off); a TrainMode = batch-statistics
+    BatchNorm that updates the running statistics in P, and DropPath with the given factors.
+    recompute: keep only each extractor's input query and recompute its internals in the backward (the reference's
+    `with_cp=True` checkpointing, dinov3_adapter.py:140-156); the values computed are the same."""
+    if gemm not in ("tf32", "fp32"):
+        raise ValueError(f"gemm tier must be 'tf32' or 'fp32', got {gemm!r}")
+    with _gemm_tier(gemm):
+        return _trainable_forward(P, variant, x, taps, num_classes, train_mode, recompute)
+
+
+def _extractor(P, p, c, feat, B, h, drop_scale):
+    """One extractor (dinov3_adapter.py:140-156, ms_deform_attn.py:158-216): c [B*Lq, D] -> c + attn, then + ffn
+    (+ drop_path(ffn) when `drop_scale` [B] is given)."""
+    Lq = h * h * 21 // 4
+    lin = lambda t, q, res=None: LinearF.apply(t, P[q + ".weight"].reshape(P[q + ".weight"].shape[0], -1), P.get(q + ".bias"), res)
+    qn = LayerNormF.apply(c, P[p + "query_norm.weight"], P[p + "query_norm.bias"], cfg.LN_EPS_ADAPTER)
+    fn = LayerNormF.apply(feat, P[p + "feat_norm.weight"], P[p + "feat_norm.bias"], cfg.LN_EPS_ADAPTER)
+    value = lin(fn, p + "attn.value_proj")
+    offaw = LinearF.apply(qn, torch.cat([P[p + "attn.sampling_offsets.weight"], P[p + "attn.attention_weights.weight"]], 0),
+                          torch.cat([P[p + "attn.sampling_offsets.bias"], P[p + "attn.attention_weights.bias"]], 0), None)
+    samp = MSDAF.apply(value, offaw, B, h, h)
+    c = lin(samp, p + "attn.output_proj", c)                    # c + attn
+    fq = LayerNormF.apply(c, P[p + "ffn_norm.weight"], P[p + "ffn_norm.bias"], cfg.LN_EPS_ADAPTER)
+    f1 = lin(fq, p + "ffn.fc1")
+    f2 = ActF.apply(DWConvF.apply(f1, P[p + "ffn.dwconv.dwconv.weight"], P[p + "ffn.dwconv.dwconv.bias"], B, h, h, 3), L.ACT_GELU)
+    if drop_scale is None:
+        return lin(f2, p + "ffn.fc2", c)                        # c + ffn
+    return DropPathAddF.apply(c, lin(f2, p + "ffn.fc2"), drop_scale, Lq)   # c + drop_path(ffn)
+
+
+def _recomputed_extractor(tier, *args):
+    """`_extractor` on the matrix-product tier of the step that ran it: the backward's replay runs after
+    `trainable_forward` has restored the module-global tier."""
+    with _gemm_tier(tier):
+        return _extractor(*args)
+
+
+def _trainable_forward(P, variant, x, taps, num_classes, train_mode=None, recompute=False):
     v = cfg.VARIANTS[variant]
     D = v.embed_dim
     B, _, S, _ = x.shape
@@ -571,23 +608,17 @@ def _trainable_forward(P, variant, x, taps, num_classes, train_mode=None):
 
     # ---- interaction blocks (dinov3_adapter.py:140-231, ms_deform_attn.py:158-216)
     names = [f"{A}interactions.{i}.extractor." for i in range(4)] + [f"{A}interactions.3.extra_extractors.{j}." for j in range(2)]
+    # with `recompute`, each extractor is one checkpointed segment from (c, tap) to the new c.  Nothing inside one draws
+    # random numbers (DropPath's factors are precomputed) or touches BatchNorm statistics, so the replay needs no RNG state
+    # and updates nothing twice.
     for e, k in enumerate((0, 1, 2, 3, 3, 3)):
-        p = names[e]
         feat = taps[k].reshape(B * h * h, D)
-        qn = LayerNormF.apply(c, P[p + "query_norm.weight"], P[p + "query_norm.bias"], cfg.LN_EPS_ADAPTER)
-        fn = LayerNormF.apply(feat, P[p + "feat_norm.weight"], P[p + "feat_norm.bias"], cfg.LN_EPS_ADAPTER)
-        value = lin(fn, p + "attn.value_proj")
-        offaw = LinearF.apply(qn, torch.cat([P[p + "attn.sampling_offsets.weight"], P[p + "attn.attention_weights.weight"]], 0),
-                              torch.cat([P[p + "attn.sampling_offsets.bias"], P[p + "attn.attention_weights.bias"]], 0), None)
-        samp = MSDAF.apply(value, offaw, B, h, h)
-        c = lin(samp, p + "attn.output_proj", c)                    # c + attn
-        fq = LayerNormF.apply(c, P[p + "ffn_norm.weight"], P[p + "ffn_norm.bias"], cfg.LN_EPS_ADAPTER)
-        f1 = lin(fq, p + "ffn.fc1")
-        f2 = ActF.apply(DWConvF.apply(f1, P[p + "ffn.dwconv.dwconv.weight"], P[p + "ffn.dwconv.dwconv.bias"], B, S16, S16, 3), L.ACT_GELU)
-        if train_mode is None:
-            c = lin(f2, p + "ffn.fc2", c)                           # c + ffn
+        drop_scale = None if train_mode is None else train_mode.drop_scale[e]
+        if recompute:
+            c = checkpoint(_recomputed_extractor, _GEMM_TIER, P, names[e], c, feat, B, h, drop_scale, use_reentrant=False,
+                           preserve_rng_state=False)
         else:
-            c = DropPathAddF.apply(c, lin(f2, p + "ffn.fc2"), train_mode.drop_scale[e], Lq)   # c + drop_path(ffn)
+            c = _extractor(P, names[e], c, feat, B, h, drop_scale)
 
     # ---- adapter tail (dinov3_adapter.py:460-482)
     c3d = c.view(B, Lq, D)

@@ -32,16 +32,22 @@ class DinoUNetTrainer(_Base):
     _dinov3_model_name = None
     _train_semantics = None
     _device_augmentation = False
+    _train_recompute = False
 
     @classmethod
     def set_network_config(cls, network_config, dinov3_pretrained_path=None, dinov3_model_name=None,
-                           adapter_type="default", train_semantics=None, device_augmentation=False):
+                           adapter_type="default", train_semantics=None, device_augmentation=False, train_recompute=False):
         """train_semantics: `DinoUNet.train_semantics` of the networks `build_network_architecture` returns ("oracle" or
         "reference"); None keeps the module default.  device_augmentation: run the training transforms on the device
-        (dinounet_b200/augmentation.py) instead of batchgenerators' worker processes; off by default."""
+        (dinounet_b200/augmentation.py) instead of batchgenerators' worker processes; off by default.  train_recompute:
+        `DinoUNet.train_recompute` of those networks, recomputing the adapter's extractors in the backward (the reference's
+        checkpointing; what lets the large variants train at a useful batch); off by default."""
+        if not isinstance(train_recompute, bool):
+            raise ValueError(f"train_recompute must be True or False, got {train_recompute!r}")
         cls._network_config = network_config
         cls._train_semantics = train_semantics
         cls._device_augmentation = bool(device_augmentation)
+        cls._train_recompute = train_recompute
         if dinov3_pretrained_path is not None:
             cls._dinov3_pretrained_path = dinov3_pretrained_path
         if dinov3_model_name is not None:
@@ -52,6 +58,7 @@ class DinoUNetTrainer(_Base):
         DinoUNetTrainer._dinov3_pretrained_path = cls._dinov3_pretrained_path
         DinoUNetTrainer._train_semantics = cls._train_semantics
         DinoUNetTrainer._device_augmentation = cls._device_augmentation
+        DinoUNetTrainer._train_recompute = cls._train_recompute
 
     @staticmethod
     def build_network_architecture(architecture_class_name: str, arch_init_kwargs: dict,
@@ -69,6 +76,7 @@ class DinoUNetTrainer(_Base):
                                    dinov3_model_name=DinoUNetTrainer._dinov3_model_name)
         if DinoUNetTrainer._train_semantics is not None:
             net.train_semantics = DinoUNetTrainer._train_semantics
+        net.train_recompute = DinoUNetTrainer._train_recompute
         return net
 
 
