@@ -14,7 +14,9 @@
 //
 // b2u_export_segment is LabelManager.apply_inference_nonlin + convert_probabilities_to_segmentation
 // (utilities/label_handling/label_handling.py:128-175) on fp16 logits: fp32 softmax over channels and the first maximum,
-// or fp32 sigmoid and `p > 0.5` painted in channel order.
+// or fp32 sigmoid and `p > 0.5` painted in channel order (export_segment.cuh, shared with the ensemble).
+// b2u_export_segment_accumulate runs the same nonlinearity and adds the probabilities into an fp32 accumulator instead
+// of writing labels: one member of a one-pass model ensemble.
 #include <cuda_fp16.h>
 
 #include <algorithm>
@@ -22,6 +24,7 @@
 
 #include "../../include/dinounet_b200.h"
 #include "common.cuh"
+#include "export_segment.cuh"
 #include "gemm_common.h"
 #include "host_util.h"
 
@@ -69,70 +72,6 @@ __global__ void export_resample_kernel(const __half* __restrict__ in, __half* __
   }
 }
 
-// fp32 sigmoid(x) > 0.5 holds exactly for x >= 2^-23: for 0 < x <= 2^-24, exp(-x) rounds to 1 - 2^-24 and 1 + that ties
-// to 2, so 1 / 2 = 0.5; at x = 2^-23, 1 / (2 - 2^-23) rounds up to 0.5 + 2^-24.  Deciding on x keeps the threshold
-// independent of the last bit of expf.
-#define B2U_SIGMOID_HALF_THRESHOLD 0x1p-23f
-
-template <int C>
-__global__ void __launch_bounds__(256) export_segment_kernel(const __half* __restrict__ logits, long long voxels,
-                                                             int mode, const int32_t* __restrict__ region_labels,
-                                                             void* __restrict__ labels, int label_bytes,
-                                                             float* __restrict__ probs) {
-  int rl[C];
-  if (mode == 1) {
-#pragma unroll
-    for (int c = 0; c < C; ++c) rl[c] = region_labels[c];
-  }
-  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
-  for (long long v = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; v < voxels; v += stride) {
-    float x[C];
-#pragma unroll
-    for (int c = 0; c < C; ++c) x[c] = __half2float(logits[c * voxels + v]);
-    int lab = 0;
-    if (mode == 0) {
-      float m = x[0];
-#pragma unroll
-      for (int c = 1; c < C; ++c) m = fmaxf(m, x[c]);
-      float s = 0.f;
-#pragma unroll
-      for (int c = 0; c < C; ++c) {
-        x[c] = expf(__fsub_rn(x[c], m));
-        s = __fadd_rn(s, x[c]);
-      }
-      float best = -1.f;
-#pragma unroll
-      for (int c = 0; c < C; ++c) {
-        const float p = __fdiv_rn(x[c], s);
-        if (probs) probs[c * voxels + v] = p;
-        if (p > best) {  // strict: the first maximum wins, as torch.argmax
-          best = p;
-          lab = c;
-        }
-      }
-    } else {
-#pragma unroll
-      for (int c = 0; c < C; ++c) {
-        if (probs) probs[c * voxels + v] = __frcp_rn(__fadd_rn(1.f, expf(-x[c])));
-        if (x[c] >= B2U_SIGMOID_HALF_THRESHOLD) lab = rl[c];
-      }
-    }
-    if (label_bytes == 1)
-      static_cast<uint8_t*>(labels)[v] = static_cast<uint8_t>(lab);
-    else
-      static_cast<uint16_t*>(labels)[v] = static_cast<uint16_t>(lab);
-  }
-}
-
-using SegmentKernel = void (*)(const __half*, long long, int, const int32_t*, void*, int, float*);
-constexpr int kMaxExportChannels = 32;
-
-template <std::size_t... I>
-static SegmentKernel segment_kernel_for(int C, std::index_sequence<I...>) {
-  static const SegmentKernel table[] = {export_segment_kernel<static_cast<int>(I) + 1>...};
-  return table[C - 1];
-}
-
 }  // namespace b2u
 
 using namespace b2u;
@@ -175,8 +114,19 @@ extern "C" int b2u_export_segment(const void* logits, int32_t C, int64_t voxels,
   if (mode == 1 && !region_labels) return set_error(-1, "b2u_export_segment: region mode needs region_labels");
   if (label_bytes != 1 && label_bytes != 2)
     return set_error(-1, "b2u_export_segment: label_bytes %d is neither 1 nor 2", label_bytes);
-  const int blocks = static_cast<int>(std::min<long long>((voxels + 255) / 256, static_cast<long long>(num_sms()) * 16));
-  segment_kernel_for(C, std::make_index_sequence<kMaxExportChannels>{})<<<blocks, 256, 0, stream>>>(
-      static_cast<const __half*>(logits), voxels, mode, region_labels, labels, label_bytes, probs);
-  return check_launch("export_segment");
+  return launch_segment<__half, false>(static_cast<const __half*>(logits), C, voxels, mode, region_labels, labels,
+                                       label_bytes, probs, 0, nullptr, 0.f, stream, "export_segment");
+}
+
+extern "C" int b2u_export_segment_accumulate(const void* logits, int32_t C, int64_t voxels, int32_t mode, float* acc,
+                                             int32_t first, b2u_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (!logits || !acc) return set_error(-1, "b2u_export_segment_accumulate: null pointer");
+  if (C < 1 || C > kMaxExportChannels)
+    return set_error(-1, "b2u_export_segment_accumulate: C=%d outside 1..%d", C, kMaxExportChannels);
+  if (voxels <= 0) return set_error(-1, "b2u_export_segment_accumulate: voxels=%lld", static_cast<long long>(voxels));
+  if (mode != 0 && mode != 1)
+    return set_error(-1, "b2u_export_segment_accumulate: mode %d is neither 0 (labels) nor 1 (regions)", mode);
+  return launch_segment<__half, true>(static_cast<const __half*>(logits), C, voxels, mode, nullptr, nullptr, 1, acc,
+                                      first, nullptr, 0.f, stream, "export_segment_accumulate");
 }

@@ -120,15 +120,10 @@ def _to_device(predicted_logits: torch.Tensor) -> torch.Tensor:
     return predicted_logits.to(dev).contiguous()
 
 
-def convert_predicted_logits_to_segmentation_with_correct_shape(predicted_logits, plans_manager, configuration_manager,
-                                                                label_manager, properties_dict: dict,
-                                                                return_probabilities: bool = False,
-                                                                num_threads_torch: int = 8):
-    """Drop-in for export_prediction.py:15-68 on fp16 logits [C, Z, h, w]: a CUDA tensor (any strides, e.g. the
-    un-padded view `SlidingWindowPredictor` returns), or a host tensor / ndarray, which is uploaded to the current device.
-    Returns the segmentation (uint8, or uint16 for >= 255 foreground labels) in the original geometry, and with
-    `return_probabilities` also the fp32 probabilities [C, *original shape].  `num_threads_torch` is accepted for the
-    reference's signature; the host work here is numpy."""
+def _checked_logits(predicted_logits, configuration_manager, label_manager, properties_dict: dict):
+    """The export's checks, all before any launch: fp16 logits [C, Z, h, w] whose channels are the label manager's
+    heads (at most MAX_EXPORT_CHANNELS), and a resampling b2u_export_resample_f16 computes.  Returns (logits tensor,
+    has_regions, in_shape, out_shape)."""
     if isinstance(predicted_logits, np.ndarray):
         predicted_logits = torch.from_numpy(predicted_logits)
     if not isinstance(predicted_logits, torch.Tensor) or predicted_logits.ndim != 4:
@@ -148,6 +143,34 @@ def convert_predicted_logits_to_segmentation_with_correct_shape(predicted_logits
     in_shape = tuple(int(s) for s in predicted_logits.shape[1:])
     out_shape = tuple(int(s) for s in properties_dict["shape_after_cropping_and_before_resampling"])
     _check_resampling(configuration_manager, properties_dict, in_shape, out_shape)
+    return predicted_logits, has_regions, in_shape, out_shape
+
+
+def _resampled_on_device(lib, logits: torch.Tensor, in_shape, out_shape, stream) -> torch.Tensor:
+    """The fp16 logits on the target grid (b2u_export_resample_f16; unchanged when the grid is)."""
+    C = int(logits.shape[0])
+    Z, h, w = in_shape
+    _, H, W = out_shape
+    if (h, w) == (H, W):
+        return logits
+    resampled = torch.empty((C, Z, H, W), dtype=torch.float16, device=logits.device)
+    L.check(lib.b2u_export_resample_f16(logits.data_ptr(), resampled.data_ptr(), C, Z, h, w, H, W, stream),
+            "b2u_export_resample_f16")
+    return resampled
+
+
+def convert_predicted_logits_to_segmentation_with_correct_shape(predicted_logits, plans_manager, configuration_manager,
+                                                                label_manager, properties_dict: dict,
+                                                                return_probabilities: bool = False,
+                                                                num_threads_torch: int = 8):
+    """Drop-in for export_prediction.py:15-68 on fp16 logits [C, Z, h, w]: a CUDA tensor (any strides, e.g. the
+    un-padded view `SlidingWindowPredictor` returns), or a host tensor / ndarray, which is uploaded to the current device.
+    Returns the segmentation (uint8, or uint16 for >= 255 foreground labels) in the original geometry, and with
+    `return_probabilities` also the fp32 probabilities [C, *original shape].  `num_threads_torch` is accepted for the
+    reference's signature; the host work here is numpy."""
+    predicted_logits, has_regions, in_shape, out_shape = _checked_logits(predicted_logits, configuration_manager,
+                                                                         label_manager, properties_dict)
+    C = int(predicted_logits.shape[0])
     n_fg = len(label_manager.foreground_labels)
     label_bytes = 1 if n_fg < 255 else 2
 
@@ -156,14 +179,8 @@ def convert_predicted_logits_to_segmentation_with_correct_shape(predicted_logits
     dev = logits.device
     with torch.cuda.device(dev):
         stream = torch.cuda.current_stream(dev).cuda_stream
-        Z, h, w = in_shape
-        _, H, W = out_shape
-        if (h, w) != (H, W):
-            resampled = torch.empty((C, Z, H, W), dtype=torch.float16, device=dev)
-            L.check(lib.b2u_export_resample_f16(logits.data_ptr(), resampled.data_ptr(), C, Z, h, w, H, W, stream),
-                    "b2u_export_resample_f16")
-            logits = resampled
-        voxels = Z * H * W
+        logits = _resampled_on_device(lib, logits, in_shape, out_shape, stream)
+        voxels = int(np.prod(out_shape))
         labels = torch.empty(out_shape, dtype=torch.uint8 if label_bytes == 1 else torch.int16, device=dev)
         probs = torch.empty((C, *out_shape), dtype=torch.float32, device=dev) if return_probabilities else None
         region_labels = None
@@ -182,6 +199,28 @@ def convert_predicted_logits_to_segmentation_with_correct_shape(predicted_logits
         return seg
     return seg, probabilities_to_original_geometry(probs_host, properties_dict, plans_manager.transpose_backward,
                                                    has_regions)
+
+
+def accumulate_probabilities(predicted_logits, configuration_manager, label_manager, properties_dict: dict,
+                             acc: torch.Tensor, first: bool):
+    """One member of a one-pass model ensemble: the export's resampling and softmax / sigmoid of fp16 logits
+    [C, Z, h, w], added into `acc` (fp32 [C, *shape_after_cropping_and_before_resampling], contiguous, on the logits'
+    device; `first` stores instead) by b2u_export_segment_accumulate.  The probabilities are those the export writes
+    with `return_probabilities`, before the paste into the pre-crop box."""
+    predicted_logits, has_regions, in_shape, out_shape = _checked_logits(predicted_logits, configuration_manager,
+                                                                         label_manager, properties_dict)
+    C = int(predicted_logits.shape[0])
+    if tuple(acc.shape) != (C, *out_shape) or acc.dtype != torch.float32 or not acc.is_contiguous():
+        raise ValueError(f"acc must be a contiguous fp32 {(C, *out_shape)} tensor, got {acc.dtype} {tuple(acc.shape)}")
+    lib = L.load()
+    logits = _to_device(predicted_logits)
+    dev = logits.device
+    with torch.cuda.device(dev):
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        logits = _resampled_on_device(lib, logits, in_shape, out_shape, stream)
+        L.check(lib.b2u_export_segment_accumulate(logits.data_ptr(), C, int(np.prod(out_shape)), int(has_regions),
+                                                  acc.data_ptr(), int(bool(first)), stream),
+                "b2u_export_segment_accumulate")
 
 
 def export_prediction_from_logits(predicted_array_or_file, properties_dict: dict, configuration_manager, plans_manager,

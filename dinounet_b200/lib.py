@@ -96,6 +96,9 @@ SIGNATURES = {
     "b2u_sw_finalize": [vp, vp, i32, i64, vp, vp],
     "b2u_export_resample_f16": [vp, vp, i32, i32, i32, i32, i32, i32, vp],
     "b2u_export_segment": [vp, i32, i64, i32, vp, vp, i32, vp, vp],
+    "b2u_export_segment_accumulate": [vp, i32, i64, i32, vp, i32, vp],
+    "b2u_ensemble_accumulate": [vp, i32, vp, i64, i32, vp],
+    "b2u_ensemble_segment": [vp, i32, i64, i32, i32, vp, vp, i32, vp],
     "b2u_pre_minmax_f32": [vp, i64, vp, vp, vp, vp],
     "b2u_pre_zscore": [vp, i64, i32, i32, i32, i64, i64, i64, vp, vp, vp],
     "b2u_pre_normalize": [vp, i64, i32, vp, f32, f32, f32, f32, vp],

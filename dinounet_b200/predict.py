@@ -178,10 +178,7 @@ def predict_cases(predictor, cases, save_probabilities: bool, num_writers: int):
     returns it: the segmentation, or (segmentation, probabilities) with `save_probabilities`."""
     from . import export
     from .engine import GRAPH_CAPTURE
-    from .preprocess import DevicePreprocessor
-    dev = predictor.device if predictor.device.index is not None else torch.device("cuda", torch.cuda.current_device())
-    pre = DevicePreprocessor(predictor.verbose_preprocessing, dev)
-    stream = torch.cuda.current_stream(dev)
+    stream = torch.cuda.current_stream(_device(predictor))
     pm, cm, dj = predictor.plans_manager, predictor.configuration_manager, predictor.dataset_json
 
     def write(logits, properties, ofile):
@@ -193,6 +190,22 @@ def predict_cases(predictor, cases, save_probabilities: bool, num_writers: int):
             return export.convert_predicted_logits_to_segmentation_with_correct_shape(
                 logits, pm, cm, predictor.label_manager, properties, return_probabilities=save_probabilities)
 
+    return run_cases(predictor, cases, lambda data, properties: predictor.predict_logits_from_preprocessed_data(data),
+                     write, num_writers)
+
+
+def _device(predictor) -> torch.device:
+    return predictor.device if predictor.device.index is not None else torch.device("cuda", torch.cuda.current_device())
+
+
+def run_cases(predictor, cases, predict, write, num_writers: int):
+    """The prediction loop: each case of `cases` ((image, properties, truncated output name or None)) is preprocessed
+    on the device with `predictor`'s plans, `predict(data, properties)` runs on the main thread, and
+    `write(result, properties, output name)` in one of `num_writers` writer threads, with at most two cases queued
+    beyond the writers.  Returns the writers' results in case order."""
+    from .preprocess import DevicePreprocessor
+    pre = DevicePreprocessor(predictor.verbose_preprocessing, _device(predictor))
+    pm, cm, dj = predictor.plans_manager, predictor.configuration_manager, predictor.dataset_json
     with ThreadPoolExecutor(max(1, num_writers)) as writers:
         pending = []
         for image, properties, ofile in cases:
@@ -201,9 +214,9 @@ def predict_cases(predictor, cases, save_probabilities: bool, num_writers: int):
             if predictor.verbose:
                 print(f"predicting {os.path.basename(ofile) if ofile is not None else 'image'} of shape {image.shape}")
             data, _ = pre.run_case_npy(image, None, properties, pm, cm, dj)
-            logits = predictor.predict_logits_from_preprocessed_data(data)
-            pending.append(writers.submit(write, logits, properties, ofile))
-            del logits, data
+            result = predict(data, properties)
+            pending.append(writers.submit(write, result, properties, ofile))
+            del result, data
         results = [p.result() for p in pending]
     return results
 
@@ -236,6 +249,25 @@ def predict_from_files(predictor, list_of_lists_or_source_folder, output_folder_
                        num_processes_segmentation_export: int = DEFAULT_NUM_PROCESSES,
                        folder_with_segs_from_prev_stage: str = None, num_parts: int = 1, part_id: int = 0):
     check_no_previous_stage(predictor, folder_with_segs_from_prev_stage)
+    args = dict(list_of_lists_or_source_folder=list_of_lists_or_source_folder,
+                output_folder_or_list_of_truncated_output_files=output_folder_or_list_of_truncated_output_files,
+                save_probabilities=save_probabilities, overwrite=overwrite,
+                num_processes_preprocessing=num_processes_preprocessing,
+                num_processes_segmentation_export=num_processes_segmentation_export,
+                folder_with_segs_from_prev_stage=folder_with_segs_from_prev_stage, num_parts=num_parts, part_id=part_id)
+    cases = cases_from_files(predictor, list_of_lists_or_source_folder, output_folder_or_list_of_truncated_output_files,
+                             save_probabilities, overwrite, num_processes_preprocessing, num_parts, part_id, args)
+    if cases is None:
+        return None
+    return predict_cases(predictor, cases, save_probabilities, num_processes_segmentation_export)
+
+
+def cases_from_files(predictor, list_of_lists_or_source_folder, output_folder_or_list_of_truncated_output_files,
+                     save_probabilities: bool, overwrite: bool, num_processes_preprocessing: int, num_parts: int,
+                     part_id: int, args: dict):
+    """The file side of `predict_from_files`: writes `args`, `dataset.json` and `plans.json` to the output folder,
+    selects this part's cases (skipping finished ones unless `overwrite`) and returns the read-ahead generator of
+    (image, properties, truncated output name or None) that `run_cases` takes, or None when no case is left."""
     outputs = output_folder_or_list_of_truncated_output_files
     if isinstance(outputs, str):
         output_folder = outputs
@@ -244,12 +276,6 @@ def predict_from_files(predictor, list_of_lists_or_source_folder, output_folder_
     else:
         output_folder = None
     if output_folder is not None:
-        args = dict(list_of_lists_or_source_folder=list_of_lists_or_source_folder,
-                    output_folder_or_list_of_truncated_output_files=outputs, save_probabilities=save_probabilities,
-                    overwrite=overwrite, num_processes_preprocessing=num_processes_preprocessing,
-                    num_processes_segmentation_export=num_processes_segmentation_export,
-                    folder_with_segs_from_prev_stage=folder_with_segs_from_prev_stage, num_parts=num_parts,
-                    part_id=part_id)
         os.makedirs(output_folder, exist_ok=True)
         _save_json(_jsonable(copy.deepcopy(args)), os.path.join(output_folder, "predict_from_raw_data_args.json"))
         _save_json(predictor.dataset_json, os.path.join(output_folder, "dataset.json"), sort_keys=False)
@@ -268,8 +294,7 @@ def predict_from_files(predictor, list_of_lists_or_source_folder, output_folder_
         data, properties = rw.read_images(files)
         return np.asarray(data, dtype=np.float32), properties, ofile
 
-    cases = _read_ahead(read, list(zip(lists, ofiles)), num_processes_preprocessing)
-    return predict_cases(predictor, cases, save_probabilities, num_processes_segmentation_export)
+    return _read_ahead(read, list(zip(lists, ofiles)), num_processes_preprocessing)
 
 
 def predict_from_list_of_npy_arrays(predictor, image_or_list_of_images, segs_from_prev_stage_or_list_of_segs_from_prev_stage,

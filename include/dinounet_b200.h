@@ -217,11 +217,28 @@ int b2u_sw_finalize(void* acc, const void* npred, int32_t C, int64_t plane, int3
  * b2u_export_segment: fp16 logits [C, voxels], 1 <= C <= 32.  mode 0 (label maps): fp32 softmax over C, labels = index
  *   of the first maximum probability.  mode 1 (regions): fp32 sigmoid, labels = region_labels[i] (DEVICE int32 [C]) of
  *   the last channel i with p > 0.5, else 0 (label_handling.py:128-175).  labels: uint8 (label_bytes 1) or uint16 (2)
- *   [voxels]; probs: fp32 [C, voxels], written only when non-NULL.  No atomics: repeated launches give identical bits. */
+ *   [voxels]; probs: fp32 [C, voxels], written only when non-NULL.  No atomics: repeated launches give identical bits.
+ * b2u_export_segment_accumulate: the same softmax / sigmoid of fp16 logits [C, voxels], added into the fp32
+ *   accumulator acc [C, voxels] (first != 0: stored), no labels: one member of a one-pass model ensemble, whose sum
+ *   b2u_ensemble_segment then averages and segments. */
 int b2u_export_resample_f16(const void* in, void* out, int32_t C, int32_t Z, int32_t h, int32_t w, int32_t H, int32_t W,
                             b2u_stream_t stream);
 int b2u_export_segment(const void* logits, int32_t C, int64_t voxels, int32_t mode, const int32_t* region_labels,
                        void* labels, int32_t label_bytes, float* probs, b2u_stream_t stream);
+int b2u_export_segment_accumulate(const void* logits, int32_t C, int64_t voxels, int32_t mode, float* acc,
+                                  int32_t first, b2u_stream_t stream);
+
+/* ---- Ensembling saved probabilities (ensembling/ensemble.py:17-46, `merge_files`).
+ * b2u_ensemble_accumulate: acc[i] = float(src[i]) (first != 0) or acc[i] + float(src[i]) (one fp32 add) for i < n;
+ *   src fp16 (src_bytes 2) or fp32 (4).  Bit-identical to numpy's `average_probabilities` sum in member order.
+ * b2u_ensemble_segment: acc [C, voxels] /= n_members in place (one correctly rounded fp32 division: the average the
+ *   reference saves), then `convert_logits_to_segmentation` of the average into labels (uint8 / uint16 by label_bytes),
+ *   as b2u_export_segment does on fp32 input; 1 <= C <= 32, n_members <= 2^24.  Regions threshold the average at
+ *   x > 1.5 * 2^-24, where fp32 sigmoid(x) > 0.5 first holds. */
+int b2u_ensemble_accumulate(const void* src, int32_t src_bytes, float* acc, int64_t n, int32_t first,
+                            b2u_stream_t stream);
+int b2u_ensemble_segment(float* acc, int32_t C, int64_t voxels, int32_t n_members, int32_t mode,
+                         const int32_t* region_labels, void* labels, int32_t label_bytes, b2u_stream_t stream);
 
 /* ---- Case preprocessing (preprocessing/preprocessors/default_preprocessor.py:40-118 `run_case_npy` of a 2D
  * configuration), fp32 channels in the caller's memory.  Bit-identical to numpy / scipy for finite input.
