@@ -124,6 +124,7 @@ SIGNATURES = {
     "b2u_aug_work_bytes": [i32, i32, i32, i32, i32, i32],
     "b2u_aug_apply": [vp, vp, i32, i32, i32, i32, i32, i32, vp, vp, C.c_uint64, vp, i32, vp, vp, vp, vp],
     "b2u_aug_noise_field": [C.c_uint64, i32, i32, i64, vp, vp],
+    "b2u_dl_crop": [vp, vp, i32, i32, i32, i32, i32, vp, i32, vp, vp, vp],
     "b2u_dice_ce_work_doubles": [i32, i32, i64, i32],
     "b2u_dice_ce_stats": [vp, vp, i32, i32, i32, vp, vp, vp, i32, i32, i64, vp],
     "b2u_dice_ce_finalize": [vp, vp, vp, vp, i32, i32, i64, i32, f32, f32, i32, i32, f32, vp],

@@ -33,21 +33,31 @@ class DinoUNetTrainer(_Base):
     _train_semantics = None
     _device_augmentation = False
     _train_recompute = False
+    _device_dataloading = False
 
     @classmethod
     def set_network_config(cls, network_config, dinov3_pretrained_path=None, dinov3_model_name=None,
-                           adapter_type="default", train_semantics=None, device_augmentation=False, train_recompute=False):
+                           adapter_type="default", train_semantics=None, device_augmentation=False, train_recompute=False,
+                           device_dataloading=False):
         """train_semantics: `DinoUNet.train_semantics` of the networks `build_network_architecture` returns ("oracle" or
         "reference"); None keeps the module default.  device_augmentation: run the training transforms on the device
         (dinounet_b200/augmentation.py) instead of batchgenerators' worker processes; off by default.  train_recompute:
         `DinoUNet.train_recompute` of those networks, recomputing the adapter's extractors in the backward (the reference's
-        checkpointing; what lets the large variants train at a useful batch); off by default."""
+        checkpointing; what lets the large variants train at a useful batch); off by default.  device_dataloading: draw
+        the 2-D batches in one read-ahead thread and assemble them on the device (dinounet_b200/dataloading.py) instead
+        of batchgenerators' worker processes; needs device_augmentation, off by default."""
         if not isinstance(train_recompute, bool):
             raise ValueError(f"train_recompute must be True or False, got {train_recompute!r}")
+        if not isinstance(device_dataloading, bool):
+            raise ValueError(f"device_dataloading must be True or False, got {device_dataloading!r}")
+        if device_dataloading and not device_augmentation:
+            raise ValueError("device_dataloading=True needs device_augmentation=True: the host transforms cannot take "
+                             "the device loader's CUDA tensors")
         cls._network_config = network_config
         cls._train_semantics = train_semantics
         cls._device_augmentation = bool(device_augmentation)
         cls._train_recompute = train_recompute
+        cls._device_dataloading = device_dataloading
         if dinov3_pretrained_path is not None:
             cls._dinov3_pretrained_path = dinov3_pretrained_path
         if dinov3_model_name is not None:
@@ -59,6 +69,7 @@ class DinoUNetTrainer(_Base):
         DinoUNetTrainer._train_semantics = cls._train_semantics
         DinoUNetTrainer._device_augmentation = cls._device_augmentation
         DinoUNetTrainer._train_recompute = cls._train_recompute
+        DinoUNetTrainer._device_dataloading = cls._device_dataloading
 
     @staticmethod
     def build_network_architecture(architecture_class_name: str, arch_init_kwargs: dict,
@@ -113,6 +124,46 @@ class DinoUNetTrainer(_Base):
 
     # None: fresh entropy per run; an int makes every rank's draws reproducible
     _device_augmentation_seed = None
+
+    # ---- data loading on the device (nnUNetTrainer.py:652-690)
+    def get_dataloaders(self):
+        """With device data loading on: a train loader at the initial patch size and a val loader at the patch size
+        (with the trainer's regions and ignore label) in this process, each with one read-ahead thread; otherwise the
+        reference's augmenters.  Under DDP each rank seeds its own loaders from `_device_dataloading_seed` and its
+        rank."""
+        if not DinoUNetTrainer._device_dataloading:
+            return _Base.get_dataloaders(self)
+        from .dataloading import DeviceDataLoader2D
+        patch_size = self.configuration_manager.patch_size
+        if len(patch_size) != 2:
+            raise NotImplementedError("device data loading covers 2-D configurations only")
+        _, _, initial_patch_size, _ = self.configure_rotation_dummyDA_mirroring_and_inital_patch_size()
+        dataset_tr, dataset_val = self.get_tr_and_val_datasets()
+        lm = self.label_manager
+        rank = getattr(self, "local_rank", 0) if getattr(self, "is_ddp", False) else 0
+        seeds = [int(np.random.SeedSequence(self._device_dataloading_seed, spawn_key=(rank, i)).generate_state(1)[0])
+                 for i in (0, 1)]
+        dl_tr = DeviceDataLoader2D(dataset_tr, self.batch_size, initial_patch_size, patch_size, lm,
+                                   oversample_foreground_percent=self.oversample_foreground_percent, mode="train",
+                                   seed=seeds[0], device=self.device)
+        dl_val = DeviceDataLoader2D(dataset_val, self.batch_size, patch_size, patch_size, lm,
+                                    oversample_foreground_percent=self.oversample_foreground_percent, mode="val",
+                                    regions=lm.foreground_regions if lm.has_regions else None,
+                                    ignore_label=lm.ignore_label, seed=seeds[1], device=self.device)
+        return dl_tr, dl_val
+
+    # None: fresh entropy per run; an int makes every rank's batches reproducible
+    _device_dataloading_seed = None
+
+    def on_train_end(self):
+        """Stops the device loaders' read-ahead threads, then the reference's end of training."""
+        from .dataloading import DeviceDataLoader2D
+        for dl in (getattr(self, "dataloader_train", None), getattr(self, "dataloader_val", None)):
+            if isinstance(dl, DeviceDataLoader2D):
+                dl.close()
+        base = getattr(super(), "on_train_end", None)   # absent without the reference package
+        if base is not None:
+            base()
 
     # ---- forward-only callers of the path that the trainer owns (nnUNetTrainer.py:355-365, :945-1005)
     def _build_loss(self):

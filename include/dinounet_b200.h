@@ -373,6 +373,20 @@ int b2u_aug_apply(const float* data, const int16_t* seg, int32_t B, int32_t C, i
                   void* work, float* out, float* target, b2u_stream_t stream);
 int b2u_aug_noise_field(uint64_t seed, int32_t B, int32_t C, int64_t n, double* out, b2u_stream_t stream);
 
+/* ---- 2-D training and validation batches from staged slice boxes (nnUNetDataLoader2D.generate_train_batch,
+ * data_loader_2d.py:7-91, get_bbox, base_data_loader.py:64-134, and the validation transforms, nnUNetTrainer.py:778-805;
+ * dinounet_b200/dataloading.py draws the boxes and stages them).
+ * b2u_dl_crop: staged: DEVICE bytes holding, per sample b, the valid part of its box: data fp32 [C, h, w] at byte offset
+ *   desc[b][0] (4-byte aligned) and seg [h, w] (int8 when desc[b][6] = 1, int16 when 2) at desc[b][1].  desc: DEVICE
+ *   int64 [B, B2U_DL_DESC] {data offset, seg offset, y0, x0, h, w, seg bytes, 0}: the box sits at rows y0 .. y0+h, columns
+ *   x0 .. x0+w of the H x W patch.  Writes data fp32 [B, C, H, W] (0 outside the box) and target: mode 0 (train) int16
+ *   [B, 1, H, W] (the stored labels, -1 outside); mode 1 (val) fp32, label -1 mapped to 0, then the label map
+ *   [B, 1, H, W] (R = 0) or R region planes [B, R, H, W] from regions: DEVICE int32 [R + 1 offsets, labels] as for
+ *   b2u_aug_apply.  B*C <= 65535.  One launch. */
+#define B2U_DL_DESC 8
+int b2u_dl_crop(const void* staged, const int64_t* desc, int32_t B, int32_t C, int32_t H, int32_t W, int32_t mode,
+                const int32_t* regions, int32_t R, float* data, void* target, b2u_stream_t stream);
+
 /* ---- Dice + cross-entropy loss and online-validation statistics on the logits of the forward path
  * (training/loss/compound_losses.py:31-56 `DC_and_CE_loss`, dice.py:72-119 `MemoryEfficientSoftDiceLoss`,
  * robust_ce_loss.py:12-16, built at nnUNetTrainer.py:363-365; consumer nnUNetTrainer.py:961-1005 `validation_step`).
