@@ -6,6 +6,9 @@ import torch
 from dinounet_b200 import lib as L
 
 TD = {L.F16: torch.float16, L.BF16: torch.bfloat16}
+U = 2.0 ** -24                       # unit roundoff of fp32
+MANT = {L.BF16: 7, L.F16: 10}        # stored mantissa bits
+EMIN = {L.BF16: -126, L.F16: -14}    # smallest normal exponent (below it the spacing stays 2^(EMIN - MANT))
 
 
 def stream():
@@ -43,3 +46,36 @@ def gemm(A, W, out, dtype, *, M=None, K=None, lda=None, N=None, ldc=None, out_fp
 def rel_err(a, b):
     a, b = a.float(), b.float()
     return ((a - b).abs().max() / b.abs().max().clamp_min(1e-12)).item()
+
+
+# ---- per-element comparison against a float64 reference (test_gpu_forward_kernels.py, test_gpu_tc_kernels.py)
+def ulp16(x, dtype):
+    """Spacing of the 16-bit type at |x| (float64)."""
+    a = x.double().abs()
+    e = torch.frexp(a)[1].double() - 1          # a = m * 2^e, 1 <= m < 2
+    e = torch.where(a > 0, e, torch.full_like(e, EMIN[dtype])).clamp_min(EMIN[dtype])
+    return torch.exp2(e - MANT[dtype])
+
+
+def bar16(ref, prop, dtype):
+    """Bar for a 16-bit output whose fp32 value is within `prop` of ref: the rounding (half an ulp, but up to a whole ulp
+    at |ref| when the value rounds across a power of two) plus prop."""
+    return ulp16(ref.abs() + prop, dtype) + prop
+
+
+def check(worst, kernel, what, got, ref, bar):
+    """|got - ref| <= bar for every element (all finite); records the worst ratio of `kernel` in the dict `worst`."""
+    got, ref = got.double(), ref.double()
+    bar = bar.double().expand_as(ref)
+    assert torch.isfinite(got).all(), f"{what}: {int((~torch.isfinite(got)).sum())} non-finite outputs"
+    ratio = (got - ref).abs() / bar
+    w = ratio.max().item() if ratio.numel() else 0.0
+    worst[kernel] = max(worst.get(kernel, 0.0), w)
+    if w > 1.0:
+        i = int(ratio.flatten().argmax())
+        idx = tuple(int(t) for t in torch.unravel_index(torch.tensor(i), ratio.shape))
+        nbad = int((ratio > 1.0).sum())
+        raise AssertionError(f"{what}: {nbad} of {ratio.numel()} elements over the bar; worst at {idx}: got "
+                             f"{got.flatten()[i].item():.9g}, ref {ref.flatten()[i].item():.9g}, bar "
+                             f"{bar.flatten()[i].item():.3g} ({w:.1f}x)")
+    return w

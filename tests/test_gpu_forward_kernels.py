@@ -22,15 +22,13 @@ import torch.nn.functional as F
 from dinounet_b200 import config as cfg
 from dinounet_b200 import lib as L
 from oracle import dinounet_oracle as O
-from tests.gpu_helpers import TD, P, stream
+from tests.gpu_helpers import TD, U, P, check, stream, ulp16
+from tests.gpu_helpers import bar16 as _bar16
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
 DTYPES = [L.BF16, L.F16]
 DNAME = {L.BF16: "bf16", L.F16: "f16"}
-U = 2.0 ** -24                       # unit roundoff of fp32
-MANT = {L.BF16: 7, L.F16: 10}        # stored mantissa bits
-EMIN = {L.BF16: -126, L.F16: -14}    # smallest normal exponent (below it the spacing stays 2^(EMIN - MANT))
 GELU_SLOPE = 1.13                    # sup |GELU'(x)| = 1.1289 (at x = sqrt(2))
 _WORST: dict = {}
 _NOTES: list = []
@@ -44,20 +42,6 @@ def _report():
         print(f"  {k:22s} {_WORST[k]:.3f}")
     for n in _NOTES:
         print("  " + n)
-
-
-def ulp16(x, dtype):
-    """Spacing of the 16-bit type at |x| (float64)."""
-    a = x.double().abs()
-    e = torch.frexp(a)[1].double() - 1          # a = m * 2^e, 1 <= m < 2
-    e = torch.where(a > 0, e, torch.full_like(e, EMIN[dtype])).clamp_min(EMIN[dtype])
-    return torch.exp2(e - MANT[dtype])
-
-
-def _bar16(ref, prop, dtype):
-    """Bar for a 16-bit output whose fp32 value is within `prop` of ref: the rounding (half an ulp, but up to a whole ulp
-    at |ref| when the value rounds across a power of two) plus prop."""
-    return ulp16(ref.abs() + prop, dtype) + prop
 
 
 def _r16(x, dtype):
@@ -77,20 +61,7 @@ def _nan(shape, dt):
 
 
 def _check(kernel, what, got, ref, bar):
-    got, ref = got.double(), ref.double()
-    bar = bar.double().expand_as(ref)
-    assert torch.isfinite(got).all(), f"{what}: {int((~torch.isfinite(got)).sum())} non-finite outputs"
-    ratio = (got - ref).abs() / bar
-    worst = ratio.max().item() if ratio.numel() else 0.0
-    _WORST[kernel] = max(_WORST.get(kernel, 0.0), worst)
-    if worst > 1.0:
-        i = int(ratio.flatten().argmax())
-        idx = tuple(int(t) for t in torch.unravel_index(torch.tensor(i), ratio.shape))
-        nbad = int((ratio > 1.0).sum())
-        raise AssertionError(f"{what}: {nbad} of {ratio.numel()} elements over the bar; worst at {idx}: got "
-                             f"{got.flatten()[i].item():.9g}, ref {ref.flatten()[i].item():.9g}, bar "
-                             f"{bar.flatten()[i].item():.3g} ({worst:.1f}x)")
-    return worst
+    return check(_WORST, kernel, what, got, ref, bar)
 
 
 def _call(fn, *args):
@@ -783,23 +754,21 @@ def _covered():
     }
 
 
-# launches whose kernels other files test at production shapes (test_gpu_gemm_overlap.py, test_gpu_attention_persistent.py)
-_ELSEWHERE = {"b2u_gemm", "b2u_qkv_rope", "b2u_attention_tc", "b2u_attention_tc_hd", "b2u_attention_rows"}
-
-
 @pytest.mark.parametrize("variant", ["dinounet_s", "dinounet_b", "dinounet_l"])
 def test_engine_shapes_are_covered(variant):
     """Builds the engine's real launch plan at (B=2, S=512) and checks that every non-GEMM, non-attention launch has its
     shape arguments in this file's case tables, so a change of the plan's shapes names the kernel whose tests no longer
-    cover it."""
+    cover it.  The tensor-core GEMM, QKV and attention launches are guarded the same way, with their epilogue signatures,
+    by test_gpu_tc_kernels.py::test_plan_shapes_are_covered."""
     from dinounet_b200.engine import ForwardEngine
+    from tests.test_gpu_tc_kernels import TC_ENTRY_POINTS
     eng = ForwardEngine(variant, O.make_state_dict(variant, 2, seed=0), 2, torch.device(DEV))
     plan, _ = eng.build_plan(B2, 512)
     tables = _covered()
     missing, n = [], 0
     for name, fn, args in plan.calls:
         fname = fn.__name__
-        if fname in _ELSEWHERE:
+        if fname in TC_ENTRY_POINTS:
             continue
         k = _key(fname, args)
         assert k is not None, f"{name}: {fname} has no case table in this file"
