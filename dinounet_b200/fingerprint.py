@@ -305,6 +305,10 @@ class DeviceFingerprintExtractor:
     def run(self, overwrite_existing: bool = False) -> dict:
         """The reference's `run` (lines 107-194): `<nnUNet_preprocessed>/<dataset>/dataset_fingerprint.json`, written
         with sort_keys and indent 4 (or loaded when it exists and overwrite_existing is False)."""
+        return self._run(overwrite_existing)
+
+    def _run(self, overwrite_existing: bool, check=None) -> dict:
+        """`run`, with `check` (integrity._FusedCheck) verifying the dataset in the same read of each case."""
         _, preprocessed = PP._raw_and_preprocessed()
         out_folder = os.path.join(preprocessed, self.dataset_name)
         os.makedirs(out_folder, exist_ok=True)
@@ -315,7 +319,7 @@ class DeviceFingerprintExtractor:
         keys = list(self.dataset.keys())
         rw_class = _determine_reader_writer(self.dataset_json, self.dataset[keys[0]]["images"][0])
         num_samples = int(self.num_foreground_voxels_for_intensitystats // len(self.dataset))
-        shapes, spacings, vectors, total, promoted = self._sample_dataset(keys, rw_class, num_samples)
+        shapes, spacings, vectors, total, promoted = self._sample_dataset(keys, rw_class, num_samples, check)
         num_channels = len(self.dataset_json["channel_names"].keys() if "channel_names" in self.dataset_json.keys()
                            else self.dataset_json["modality"].keys())
         if total == 0:
@@ -347,14 +351,20 @@ class DeviceFingerprintExtractor:
             raise
         return fingerprint
 
-    def _sample_dataset(self, keys, rw_class, num_samples):
+    def _sample_dataset(self, keys, rw_class, num_samples, check=None):
         """Reads and checks the cases ahead on `num_processes` threads and processes them in order on the current
         device: each case's draws run on the host while the device uploads and compacts the next case.  Returns
         (shapes, spacings, the dataset vectors fp32 [C, cap], the samples written per channel, whether the
-        concatenation promotes)."""
+        concatenation promotes).  With `check`, every case is also verified on its device copy, the cases are
+        sampled only while the check and the fingerprint's own checks pass, and `check.finish()` reports (and
+        raises) before anything is returned."""
         def read(k):   # and check, off the thread that drives the device
             rw = rw_class()
             images, props = rw.read_images(self.dataset[k]["images"])
+            if check is not None:
+                seg, props_seg = rw.read_seg(self.dataset[k]["label"])
+                seg, images, _ = _as_input(seg, images)
+                return images, seg, props, check.read(images, seg, props_seg)
             seg, _ = rw.read_seg(self.dataset[k]["label"])
             seg, images, _ = _as_input(seg, images)
             return images, seg, props, check_case(seg, images)
@@ -380,8 +390,12 @@ class DeviceFingerprintExtractor:
                     if vectors is None:
                         vectors = torch.empty((images.shape[0], num_samples * len(keys)), dtype=torch.float32,
                                               device=dev)
-                    case = _Case(seg, images, code, dev, lib, stream)
-                if pending is not None:   # the previous case's draws, while the device compacts this one
+                    if check is None:
+                        case = _Case(seg, images, code, dev, lib, stream)
+                    else:
+                        case = check.case(k, images, seg, props, code,
+                                          lambda c: _Case(seg, images, c, dev, lib, stream))
+                if pending is not None and (check is None or check.sampling):   # the previous case's draws, while the device compacts this one
                     count = pending.count()
                     if count == 0:
                         promoted = True
@@ -390,6 +404,8 @@ class DeviceFingerprintExtractor:
                         pending.gather_samples(ranks, vectors, total)
                         total += num_samples
                 pending = case
+            if check is not None:
+                check.finish()
         return shapes, spacings, vectors, total, promoted
 
 

@@ -117,6 +117,7 @@ SIGNATURES = {
     "b2u_fp_select": [vp, i64, vp, i32, vp, vp, vp],
     "b2u_fp_moments_work_bytes": [i64, i32],
     "b2u_fp_moments": [vp, i64, i32, i32, vp, vp, vp],
+    "b2u_vi_scan": [vp, i64, vp, i32, i64, i64, i64, vp, vp],
     "b2u_eval_masks": [vp, i32, vp, i32, i32, i32, i32, i32, C.POINTER(C.c_int64), i32, i32, i64, vp, vp, vp, vp],
     "b2u_eval_edt": [vp, i32, i32, i32, C.c_double, C.c_double, C.c_double, vp, vp, vp, vp],
     "b2u_eval_sum_f64": [vp, i64, vp, vp],

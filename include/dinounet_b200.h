@@ -319,6 +319,21 @@ int64_t b2u_fp_moments_work_bytes(int64_t n, int32_t f64);
 int b2u_fp_moments(const float* x, int64_t n, int32_t f64, int32_t with_std, void* work, void* stats,
                    b2u_stream_t stream);
 
+/* ---- Dataset integrity (experiment_planning/verify_dataset_integrity.py:32-116: the array checks of `verify_labels`
+ * and `check_cases`).
+ * b2u_vi_scan: one read of a case.  img: DEVICE fp32 [n_img] (every channel; may be null when n_img is 0); seg: DEVICE
+ *   [n_seg] in its stored dtype (B2U_EVAL_* code, naturally aligned), 1 <= n_seg < 2^31.  *result (DEVICE) is
+ *   overwritten: offenders = the seg voxels that are not an integral value in [lo, hi] (NaN included, -0.0 is 0), and
+ *   flags = B2U_VI_IMAGE_NAN / B2U_VI_IMAGE_INF (any NaN / +-inf in img) | B2U_VI_SEG_NAN (any NaN in a float32 seg). */
+typedef struct {
+  uint64_t offenders;
+  uint32_t flags;
+  uint32_t reserved;
+} b2u_vi_result;
+enum { B2U_VI_IMAGE_NAN = 1, B2U_VI_IMAGE_INF = 2, B2U_VI_SEG_NAN = 4 };
+int b2u_vi_scan(const float* img, int64_t n_img, const void* seg, int32_t dtype, int64_t n_seg, int64_t lo, int64_t hi,
+                b2u_vi_result* result, b2u_stream_t stream);
+
 /* ---- Evaluation of predictions against the ground truth (evaluation/evaluate_predictions.py:152-230
  * `compute_metrics`, HD95 / ASD as medpy's hd95 / asd).  Volumes are C-contiguous [Z, Y, X] (a mask of rank 1 or 2 is
  * padded with leading axes of size 1, and `ndim` names its true rank).
