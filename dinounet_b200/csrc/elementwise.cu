@@ -931,7 +931,7 @@ __global__ void __launch_bounds__(256) seg_head_kernel(const T* __restrict__ x, 
                                                        int rows, int ncls) {
   pdl_begin();
   __shared__ float s_a[C], s_b[C];       // per-image affine: y = x*a + b
-  __shared__ float s_w[kSegMaxClasses * C], s_bias[kSegMaxClasses];
+  __shared__ float s_w[kSegMaxClasses * 32], s_bias[kSegMaxClasses];   // ncls * C <= kSegMaxClasses * 32
   const int b = blockIdx.y;
   for (int c = threadIdx.x; c < C; c += 256) {
     const float mean = sums[(static_cast<long long>(b) * C + c) * 2] / rows;
@@ -1042,14 +1042,25 @@ extern "C" int b2u_seg_head(const void* x, const float* sums, const float* gamma
                             const float* w, const float* b, float* logits, uint8_t* labels, int32_t B, int32_t rows,
                             int32_t C, int32_t ncls, int32_t dtype, b2u_stream_t stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (C != 32) return set_error(-1, "b2u_seg_head: C must be 32 (plans features_per_stage[0])");
-  if (ncls < 1 || ncls > kSegMaxClasses) return set_error(-1, "b2u_seg_head: 1 <= ncls <= %d", kSegMaxClasses);
+  // C = 32: the last decoder stage (seg_layers[-1]); 64 / 128: the deep-supervision heads on the earlier stages
+  if (C != 32 && C != 64 && C != 128) return set_error(-1, "b2u_seg_head: C must be 32, 64 or 128 (features_per_stage[:3])");
+  if (ncls < 1 || ncls * C > kSegMaxClasses * 32)
+    return set_error(-1, "b2u_seg_head: 1 <= ncls <= %d at C=%d", kSegMaxClasses * 32 / C, C);
   dim3 grid((rows + 255) / 256, B);
-  if (ncls <= 8) {
-    B2U_DISPATCH_T(dtype, (launch_pdl(seg_head_kernel8<T, 32>, grid, 256, 0, stream, static_cast<const T*>(x), sums, gamma, beta, eps, w, b, logits, labels, rows, ncls)));
-  } else {
-    B2U_DISPATCH_T(dtype, (launch_pdl(seg_head_kernel<T, 32>, grid, 256, 0, stream, static_cast<const T*>(x), sums, gamma, beta, eps, w, b, logits, labels, rows, ncls)));
+#define B2U_SEG_HEAD(CC)                                                                                                         \
+  if (ncls <= 8) {                                                                                                              \
+    B2U_DISPATCH_T(dtype, (launch_pdl(seg_head_kernel8<T, CC>, grid, 256, 0, stream, static_cast<const T*>(x), sums, gamma, beta, eps, w, b, logits, labels, rows, ncls))); \
+  } else {                                                                                                                      \
+    B2U_DISPATCH_T(dtype, (launch_pdl(seg_head_kernel<T, CC>, grid, 256, 0, stream, static_cast<const T*>(x), sums, gamma, beta, eps, w, b, logits, labels, rows, ncls))); \
   }
+  if (C == 32) {
+    B2U_SEG_HEAD(32)
+  } else if (C == 64) {
+    B2U_SEG_HEAD(64)
+  } else {
+    B2U_SEG_HEAD(128)
+  }
+#undef B2U_SEG_HEAD
   return check_launch("seg_head");
 }
 

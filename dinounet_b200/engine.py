@@ -94,6 +94,7 @@ class Plan:
         # (call index, ViT block, patch(args, sin_ptr, cos_ptr, keep) -> args) for every call that reads the RoPE tables
         self.rope_sites: list = []
         self.scaled_vit = None  # (Plan, scales buffer): the ViT section on per-block rescaled RoPE tables, built on first use
+        self.ds = None          # (Plan, [logits@S, @S/2, @S/4]): the deep-supervision forward on these buffers (`ds_plan`)
 
     def add(self, name: str, fn, *args):
         self.calls.append((name, fn, args))
@@ -311,6 +312,10 @@ class ForwardEngine:
                 w[f"d{s}.n{j}w"], w[f"d{s}.n{j}b"] = f32(P[p + "norm.weight"]), f32(P[p + "norm.bias"])
         w["seg.w"] = f32(P["decoder.seg_layers.2.weight"].reshape(self.ncls, -1))
         w["seg.b"] = f32(P["decoder.seg_layers.2.bias"])
+        for s in range(2):      # the deep-supervision heads on decoder stages 0 and 1 (read by `ds_plan` only)
+            if f"decoder.seg_layers.{s}.weight" in P:
+                w[f"ds{s}.w"] = f32(P[f"decoder.seg_layers.{s}.weight"].reshape(self.ncls, -1))
+                w[f"ds{s}.b"] = f32(P[f"decoder.seg_layers.{s}.bias"])
         return w
 
     # ------------------------------------------------------------------ plan helpers
@@ -348,9 +353,11 @@ class ForwardEngine:
 
     # ------------------------------------------------------------------ plan
     def build_plan(self, B: int, S: int, w: Optional[Dict[str, torch.Tensor]] = None,
-                   share: Optional[Dict[str, torch.Tensor]] = None) -> Tuple[Plan, dict]:
+                   share: Optional[Dict[str, torch.Tensor]] = None, ds: bool = False) -> Tuple[Plan, dict]:
         """The (B, S) launch list on the weights `w` (default: the engine's own).  With `share` (the buffers of an
-        existing (B, S) plan) every activation buffer is taken from it instead of allocated."""
+        existing (B, S) plan) every activation buffer is taken from it instead of allocated.  `ds`: also the
+        deep-supervision heads seg_layers[1] / [0] on decoder stages 1 / 0, into fp32 NCHW buffers "logits_ds1"
+        [B, ncls, S/2, S/2] and "logits_ds2" [B, ncls, S/4, S/4] that are always allocated here."""
         if S < 128 or S % 128:
             # every pyramid level (S/2 ... S/32) must tile: conv row widths multiples of 4, the halo-mode convs multiples of 8,
             # the three-plane depthwise conv S/16 % 8 == 0 -> multiples of 128 (128, 256, 384, 512, 640, ...); the reference's
@@ -617,6 +624,13 @@ class ForwardEngine:
                            bias=w[f"d{s}.c{j}b"], conv=L.CONV3X3_S1, img=(B, r_hi, r_hi, cin))
                 ss = sums_slot()
                 plan.add(f"d{s}.in{j}.stats", lib.b2u_in_stats, _ptr(CO), skip, _ptr(ss), _ptr(in_work), B, r_hi * r_hi, skip, rt)
+                if ds and s < 2 and j == 1:
+                    # dinounet_training.py:619-626: seg_layers[s] on the stage output = the seg head on the pre-norm
+                    # conv output and its statistics (16-bit activation, fp32 logits), no argmax
+                    out = bufs[f"logits_ds{2 - s}"] = torch.empty((B, self.ncls, r_hi, r_hi), dtype=torch.float32, device=dev)
+                    plan.add(f"d{s}.ds_head", lib.b2u_seg_head, _ptr(CO), _ptr(ss), _ptr(w[f"d{s}.n{j}w"]),
+                             _ptr(w[f"d{s}.n{j}b"]), cfg.IN_EPS, _ptr(w[f"ds{s}.w"]), _ptr(w[f"ds{s}.b"]), _ptr(out), None,
+                             B, r_hi * r_hi, skip, self.ncls, rt)
                 if s == 2 and j == 1:
                     plan.add("seg_head", lib.b2u_seg_head, _ptr(CO), _ptr(ss), _ptr(w[f"d{s}.n{j}w"]), _ptr(w[f"d{s}.n{j}b"]),
                              cfg.IN_EPS, _ptr(w["seg.w"]), _ptr(w["seg.b"]), _ptr(logits), _ptr(labels), B, r_hi * r_hi, skip,
@@ -647,6 +661,41 @@ class ForwardEngine:
             else:
                 self._plans[key] = self.build_plan(B, S)
         return self._plans[key]
+
+    def ds_plan(self, B: int, S: int) -> Tuple[Plan, List[torch.Tensor]]:
+        """The deep-supervision variant of the (B, S) plan (`build_plan(ds=True)` or the fp32 tier's), on the activation
+        buffers of the (B, S) plan, built on first use and dropped with it: (plan, [logits@S, logits@S/2, logits@S/4]).
+        The eval plan, its CUDA graphs and its launch list are untouched."""
+        plan, bufs = self.get_plan(B, S)
+        if plan.ds is None:
+            if "ds0.w" not in self.w:
+                raise KeyError("deep supervision needs decoder.seg_layers.0 / .1 in the packed state dict")
+            with torch.cuda.device(self.device):
+                if self.precision == "fp32":
+                    from .engine_fp32 import build_plan_fp32
+                    dp, dbufs = build_plan_fp32(self, B, S, share=bufs, ds=True)
+                else:
+                    dp, dbufs = self.build_plan(B, S, share=bufs, ds=True)
+            plan.ds = (dp, [bufs["logits"], dbufs["logits_ds1"], dbufs["logits_ds2"]])
+        return plan.ds
+
+    def forward_ds(self, x: torch.Tensor) -> List[torch.Tensor]:
+        """x: fp32 [B, 3, S, S] -> [logits@S, logits@S/2, logits@S/4] (fp32 NCHW, highest resolution first, as the
+        reference's decoder returns them with deep supervision, dinounet_training.py:627-629).  logits@S is what `forward`
+        computes.  The returned tensors are the engine's own buffers (overwritten by the next call)."""
+        if x.device.type != "cuda":
+            raise L.NativeLibraryError("dinounet_b200 runs on CUDA devices only (no CPU fallback)")
+        B, Cc, S, S_ = x.shape
+        if Cc != 3 or S != S_:
+            raise ValueError("expected [B, 3, S, S]")
+        if x.device != self.device:
+            raise ValueError(f"input on {x.device}, engine on {self.device}")
+        _, bufs = self.get_plan(B, S)
+        dp, outs = self.ds_plan(B, S)
+        bufs["x"].copy_(x, non_blocking=True)
+        with torch.cuda.device(self.device):
+            dp.run(torch.cuda.current_stream(self.device).cuda_stream)
+        return outs
 
     def clear_plans(self):
         """Frees every cached (batch, size) buffer set and CUDA graph."""

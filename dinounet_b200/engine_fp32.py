@@ -26,9 +26,10 @@ def _patch_attention_rope(args, sin: int, cos: int, keep: list):
     return (args[0], sin, cos) + tuple(args[3:])
 
 
-def build_plan_fp32(eng, B: int, S: int, w=None, share=None):
+def build_plan_fp32(eng, B: int, S: int, w=None, share=None, ds=False):
     """The (B, S) launch list of the fp32 tier on the weights `w` (default: the engine's own); with `share` (the buffers
-    of an existing (B, S) plan) every buffer is taken from it instead of allocated."""
+    of an existing (B, S) plan) every buffer is taken from it instead of allocated.  `ds`: also the deep-supervision
+    heads, as `ForwardEngine.build_plan(ds=True)`."""
     from .engine import Plan
     if S % 32 or S < 64:
         raise ValueError("fp32 tier: input size must be a multiple of 32 (>= 64)")
@@ -247,6 +248,12 @@ def build_plan_fp32(eng, B: int, S: int, w=None, share=None):
             plan.add(f"d{s}.in{j}", lib.b2u_f32_instnorm, _ptr(CO), skip, _ptr(CA), skip, _ptr(w[f"d{s}.n{j}w"]),
                      _ptr(w[f"d{s}.n{j}b"]), _ptr(in_work), _ptr(in_stats), B, r_hi * r_hi, skip, cfg.IN_EPS, 1)
             src, cin = CA, skip
+        if ds and s < 2:
+            # seg_layers[s] on the stage output (dinounet_training.py:619-626); the labels it writes are overwritten by
+            # the final head's
+            out = bufs[f"logits_ds{2 - s}"] = torch.empty((B, eng.ncls, r_hi, r_hi), dtype=f32, device=dev)
+            gemm(f"d{s}.ds_seg", CA, B * r_hi * r_hi, skip, skip, w[f"ds{s}.w"], eng.ncls, lin, eng.ncls, bias=w[f"ds{s}.b"])
+            plan.add(f"d{s}.ds_out", lib.b2u_f32_seg_out, _ptr(lin), _ptr(out), _ptr(labels), B, r_hi * r_hi, eng.ncls)
         lres, below = CA, skip
     gemm("seg", CA, B * S * S, feats[0], feats[0], w["seg.w"], eng.ncls, lin, eng.ncls, bias=w["seg.b"])
     plan.add("seg_out", lib.b2u_f32_seg_out, _ptr(lin), _ptr(logits), _ptr(labels), B, S * S, eng.ncls)

@@ -53,6 +53,17 @@ class QkvParams(C.Structure):
     ]
 
 
+class DsTargetsParams(C.Structure):
+    """b2u_ds_targets_params (deep-supervision target downsampling)."""
+    _fields_ = [
+        ("src", C.c_void_p), ("dtype", C.c_int32), ("B", C.c_int32), ("C", C.c_int32), ("H", C.c_int32), ("W", C.c_int32),
+        ("nscales", C.c_int32), ("fy", C.c_int32 * 4), ("fx", C.c_int32 * 4), ("dst", C.c_void_p * 4),
+    ]
+
+
+DS_MAX_SCALES, DS_INT16, DS_FP32 = 4, 0, 1
+
+
 class F32GemmParams(C.Structure):
     """b2u_f32_gemm_params (fp32 parity tier)."""
     _fields_ = [
@@ -126,6 +137,7 @@ SIGNATURES = {
     "b2u_aug_apply": [vp, vp, i32, i32, i32, i32, i32, i32, vp, vp, C.c_uint64, vp, i32, vp, vp, vp, vp],
     "b2u_aug_noise_field": [C.c_uint64, i32, i32, i64, vp, vp],
     "b2u_dl_crop": [vp, vp, i32, i32, i32, i32, i32, vp, i32, vp, vp, vp],
+    "b2u_ds_targets": [C.POINTER(DsTargetsParams), vp],
     "b2u_dice_ce_work_doubles": [i32, i32, i64, i32],
     "b2u_dice_ce_stats": [vp, vp, i32, i32, i32, vp, vp, vp, i32, i32, i64, vp],
     "b2u_dice_ce_finalize": [vp, vp, vp, vp, i32, i32, i64, i32, f32, f32, i32, i32, f32, vp],

@@ -259,18 +259,57 @@ class DC_and_BCE_loss(nn.Module):
         return self._run(net_output, target)[0]
 
 
+class DeepSupervisionWrapper(nn.Module):
+    """training/loss/deep_supervision.py: `loss` applied to every (output, target) pair of the lists it is given,
+    weighted by `weight_factors` (all 1 when None); a pair whose weight is 0 is not evaluated, so the head that produced
+    it gets no gradient.  Wraps the fused losses above (one fused pass per scale)."""
+
+    def __init__(self, loss, weight_factors=None):
+        super().__init__()
+        if weight_factors is not None:
+            assert any(x != 0 for x in weight_factors), "At least one weight factor should be != 0.0"
+            weight_factors = tuple(float(x) for x in weight_factors)
+        self.weight_factors = weight_factors
+        self.loss = loss
+
+    def _weights(self, n):
+        return (1.0,) * n if self.weight_factors is None else self.weight_factors
+
+    def forward(self, *args):
+        assert all(isinstance(i, (tuple, list)) for i in args), \
+            f"all args must be either tuple or list, got {[type(i) for i in args]}"
+        w = self._weights(len(args[0]))
+        return sum(w[i] * self.loss(*inputs) for i, inputs in enumerate(zip(*args)) if w[i] != 0.0)
+
+    def _run(self, net_output, target):
+        """(weighted loss over every scale, and scale 0's out3 / counts / bad): what `validation_statistics` reads."""
+        w = self._weights(len(net_output))
+        loss, first = None, None
+        for i, (o, t) in enumerate(zip(net_output, target)):
+            if w[i] == 0.0 and i > 0:
+                continue
+            r = self.loss._run(o, t)
+            if i == 0:
+                first = r
+            if w[i] != 0.0:
+                loss = w[i] * r[0] if loss is None else loss + w[i] * r[0]
+        return (loss, *first[1:])
+
+
 def validation_statistics(loss_module, net_output: torch.Tensor, target: torch.Tensor) -> Dict[str, np.ndarray]:
     """What `nnUNetTrainer.validation_step` returns for one batch (nnUNetTrainer.py:961-1005): the loss and the hard
     tp / fp / fn, float32.  Label maps (`DC_and_CE_loss`): argmax(net_output) per foreground class (background dropped),
     over the pixels not labelled with the loss's ignore label.  Regions (`DC_and_BCE_loss`): sigmoid(net_output) > 0.5 per region, each pixel weighted by 1 - t_ign when the target
     carries an ignore channel.  Under data-parallel batch Dice the loss uses the all-reduced sums; the counts stay per
-    rank (the trainer gathers them at the end of the epoch)."""
+    rank (the trainer gathers them at the end of the epoch).  With a `DeepSupervisionWrapper`, `net_output` and `target`
+    are lists: the loss is the weighted sum over the scales, the counts come from scale 0 (nnUNetTrainer.py:964-967)."""
     with torch.no_grad():
         loss, _, counts, bad = loss_module._run(net_output, target)
     counts = counts.cpu().numpy()          # synchronises
     if bad is not None and int(bad.item()):
         raise RuntimeError("target contains labels outside [0, num_classes)")
     f = counts.astype(np.float32)          # the reference sums float products
-    if isinstance(loss_module, DC_and_BCE_loss):
+    base = loss_module.loss if isinstance(loss_module, DeepSupervisionWrapper) else loss_module
+    if isinstance(base, DC_and_BCE_loss):
         return {"loss": loss.detach().cpu().numpy(), "tp_hard": f[0], "fp_hard": f[1], "fn_hard": f[2]}
     return {"loss": loss.detach().cpu().numpy(), "tp_hard": f[0, 1:], "fp_hard": f[1, 1:], "fn_hard": f[2, 1:]}

@@ -662,10 +662,9 @@ class DinoUNet(nn.Module):
                              tuple(self.encoder.target_channels), self.attn_impl, getattr(self, "query_dtype", "fp32"),
                              getattr(self, "precision", "16"))
 
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
-        if self.decoder.deep_supervision:
-            raise NotImplementedError("deep supervision outputs are not produced by the native forward path "
-                                      "(DinoUNetTrainer derives from nnUNetTrainerNoDeepSupervision)")
+    def forward(self, x: torch.Tensor):
+        """Logits [B, C, H, W] (fp32); with `decoder.deep_supervision` set, the list [logits@S, logits@S/2, logits@S/4]
+        of every decoder stage's head, highest resolution first (dinounet_training.py:603-629)."""
         if torch.is_grad_enabled() and self.training:
             # training step (nnUNetTrainer.py:899-929): frozen ViT on the engine, everything else differentiable through the
             # autograd Functions of train_path.py (forward and backward on hand-written kernels; `train_gemm` picks the
@@ -677,6 +676,8 @@ class DinoUNet(nn.Module):
         elif Cc != 3:
             x = x.repeat(1, 3 // Cc + (1 if 3 % Cc != 0 else 0), 1, 1)[:, :3] if Cc < 3 else x[:, :3]
         x = x.float().contiguous()
+        if self.decoder.deep_supervision:
+            return [t.clone() for t in self._eval_engine(x.device).forward_ds(x)]
         logits, _ = self._eval_engine(x.device).forward(x)
         return logits.clone()
 
@@ -711,7 +712,8 @@ class DinoUNet(nn.Module):
         return s, k
 
     def train_forward(self, x: torch.Tensor, *, rope_scales: torch.Tensor = None, drop_keep: torch.Tensor = None) -> torch.Tensor:
-        """Differentiable logits [B, C, H, W] (fp32): gradients for the 289 trainable tensors outside the frozen backbone.
+        """Differentiable logits [B, C, H, W] (fp32): gradients for the 289 trainable tensors outside the frozen backbone;
+        with `decoder.deep_supervision` set, the list of the three decoder heads' logits (see `forward`).
         With train_semantics == "reference", `rope_scales` [depth] (fp32 RoPE coordinate factor of each ViT block) and
         `drop_keep` [6, B] (0/1 DropPath keep flags, one row per extractor in the order interactions.0..3.extractor,
         interactions.3.extra_extractors.0..1) pin the random draws; an absent one is drawn on the model's device from
@@ -738,7 +740,8 @@ class DinoUNet(nn.Module):
             with torch.no_grad():
                 taps = self._get_engine(x.device).extract_vit_features(x)
             P = self.state_dict(keep_vars=True)
-            return trainable_forward(P, self.dinov3_model_name, x, taps, self.num_classes, gemm, recompute=recompute)
+            return trainable_forward(P, self.dinov3_model_name, x, taps, self.num_classes, gemm, recompute=recompute,
+                                     deep_supervision=bool(self.decoder.deep_supervision))
         B = x.shape[0]
         depth = cfg.VARIANTS[self.dinov3_model_name].depth
         with torch.no_grad():
@@ -755,7 +758,8 @@ class DinoUNet(nn.Module):
         P = self.state_dict(keep_vars=True)
         mode = TrainMode(bn=bn, drop_scale=(drop_keep / self._DROP_KEEP).contiguous(), sync=_bn_sync())
         self._repack_before_eval = True
-        return trainable_forward(P, self.dinov3_model_name, x, taps, self.num_classes, gemm, mode, recompute)
+        return trainable_forward(P, self.dinov3_model_name, x, taps, self.num_classes, gemm, mode, recompute,
+                                 bool(self.decoder.deep_supervision))
 
     @torch.no_grad()
     def predict_labels(self, x: torch.Tensor) -> torch.Tensor:

@@ -529,18 +529,21 @@ def _gemm_tier(tier: str):
 
 
 def trainable_forward(P: Dict[str, torch.Tensor], variant: str, x: torch.Tensor, taps: List[torch.Tensor], num_classes: int,
-                      gemm: str = "tf32", train_mode: Optional[TrainMode] = None, recompute: bool = False) -> torch.Tensor:
+                      gemm: str = "tf32", train_mode: Optional[TrainMode] = None, recompute: bool = False,
+                      deep_supervision: bool = False):
     """Differentiable forward of everything outside the frozen backbone.  P: reference-keyed parameters / buffers
     (`net.state_dict(keep_vars=True)`), x [B,3,S,S] fp32, taps: 4 x [B, P, D] fp32 (frozen ViT outputs) -> logits [B,C,S,S].
     gemm: matrix-product tier, "tf32" (tensor cores) or "fp32" (SIMT parity tier); the backward uses the same tier.
     train_mode: None = eval-mode modules (BatchNorm on running statistics, DropPath off); a TrainMode = batch-statistics
     BatchNorm that updates the running statistics in P, and DropPath with the given factors.
     recompute: keep only each extractor's input query and recompute its internals in the backward (the reference's
-    `with_cp=True` checkpointing, dinov3_adapter.py:140-156); the values computed are the same."""
+    `with_cp=True` checkpointing, dinov3_adapter.py:140-156); the values computed are the same.
+    deep_supervision: return [logits@S, logits@S/2, logits@S/4], seg_layers[2] / [1] / [0] on decoder stages 2 / 1 / 0
+    (dinounet_training.py:619-629); a head whose logits no loss term reads gets no gradient."""
     if gemm not in ("tf32", "fp32"):
         raise ValueError(f"gemm tier must be 'tf32' or 'fp32', got {gemm!r}")
     with _gemm_tier(gemm):
-        return _trainable_forward(P, variant, x, taps, num_classes, train_mode, recompute)
+        return _trainable_forward(P, variant, x, taps, num_classes, train_mode, recompute, deep_supervision)
 
 
 def _extractor(P, p, c, feat, B, h, drop_scale):
@@ -570,7 +573,7 @@ def _recomputed_extractor(tier, *args):
         return _extractor(*args)
 
 
-def _trainable_forward(P, variant, x, taps, num_classes, train_mode=None, recompute=False):
+def _trainable_forward(P, variant, x, taps, num_classes, train_mode=None, recompute=False, deep_supervision=False):
     v = cfg.VARIANTS[variant]
     D = v.embed_dim
     B, _, S, _ = x.shape
@@ -659,6 +662,7 @@ def _trainable_forward(P, variant, x, taps, num_classes, train_mode=None, recomp
 
     # ---- decoder (dinounet_training.py:603-629)
     lres = skips[3]
+    outs = []
     for s in range(3):
         skip_c = (128, 64, 32)[s]
         r_lo = S8 << s
@@ -670,8 +674,12 @@ def _trainable_forward(P, variant, x, taps, num_classes, train_mode=None, recomp
             t = Conv3x3F.apply(t, P[p + "conv.weight"], P[p + "conv.bias"], B, r_hi, r_hi, 1)
             t = InstNormLReLUF.apply(t, P[p + "norm.weight"], P[p + "norm.bias"], B, r_hi * r_hi)
         lres = t
-    logits = lin(lres, "decoder.seg_layers.2")
-    return logits.view(B, S, S, num_classes).permute(0, 3, 1, 2).contiguous()
+        if deep_supervision or s == 2:
+            y = lin(t, f"decoder.seg_layers.{s}")
+            outs.append(y.view(B, r_hi, r_hi, num_classes).permute(0, 3, 1, 2).contiguous())
+    if deep_supervision:
+        return outs[::-1]
+    return outs[0]
 
 
 class AddF(Function):

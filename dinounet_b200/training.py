@@ -17,7 +17,8 @@ from torch import distributed as dist
 from torch import nn
 
 from . import config as cfg
-from .loss import DC_and_BCE_loss, DC_and_CE_loss, validation_statistics
+from . import deep_supervision as DS
+from .loss import DC_and_BCE_loss, DC_and_CE_loss, DeepSupervisionWrapper, validation_statistics
 from .network_architecture import DinoUNet
 
 try:  # the reference package (needs batchgenerators etc.); optional
@@ -170,14 +171,49 @@ class DinoUNetTrainer(_Base):
         """The fused native losses with the reference's arguments.  Region-based datasets: sigmoid Dice (batch_dice from
         the plans, every region, smooth 1e-5) + BCE, ignore channel when the dataset has an ignore label.  Label maps:
         Dice (no background) + CE, weights 1:1.  `ddp` follows the trainer, so under DDP the batch Dice sums are taken
-        over every rank.  No deep-supervision wrapper (the trainer derives from nnUNetTrainerNoDeepSupervision)."""
+        over every rank.  With `enable_deep_supervision` (off in the base trainer, which derives from
+        nnUNetTrainerNoDeepSupervision; a subclass sets it in its constructor) the loss is wrapped in a
+        `DeepSupervisionWrapper` with the reference's weights (nnUNetTrainer.py:370-390); a plan whose scales do not
+        match the network's three outputs raises here, before training starts."""
         if self.label_manager.has_regions:
-            return DC_and_BCE_loss({}, {"batch_dice": self.configuration_manager.batch_dice, "do_bg": True,
+            loss = DC_and_BCE_loss({}, {"batch_dice": self.configuration_manager.batch_dice, "do_bg": True,
                                         "smooth": 1e-5, "ddp": self.is_ddp},
                                    use_ignore_label=self.label_manager.ignore_label is not None)
-        return DC_and_CE_loss({"batch_dice": self.configuration_manager.batch_dice, "smooth": 1e-5, "do_bg": False,
-                               "ddp": self.is_ddp}, {}, weight_ce=1, weight_dice=1,
-                              ignore_label=self.label_manager.ignore_label)
+        else:
+            loss = DC_and_CE_loss({"batch_dice": self.configuration_manager.batch_dice, "smooth": 1e-5, "do_bg": False,
+                                   "ddp": self.is_ddp}, {}, weight_ce=1, weight_dice=1,
+                                  ignore_label=self.label_manager.ignore_label)
+        if getattr(self, "enable_deep_supervision", False):
+            weights = DS.deep_supervision_weights(len(self._ds_scales()), self.is_ddp)
+            loss = DeepSupervisionWrapper(loss, weights)
+        return loss
+
+    def _ds_scales(self):
+        """The plan's deep-supervision scales (nnUNetTrainer.py:300-306), checked against the network's outputs."""
+        return DS.deep_supervision_scales(self.configuration_manager.pool_op_kernel_sizes)
+
+    def _target_to_device(self, target, keep_list: bool):
+        """The batch's target on the device: the list of the host transforms' scales when `keep_list`, else its first
+        (full-resolution) entry."""
+        if isinstance(target, list):
+            if keep_list:
+                return [t.to(self.device, non_blocking=True) for t in target]
+            target = target[0]
+        return target.to(self.device, non_blocking=True)
+
+    def _ds_targets(self, target):
+        """With deep supervision, a target made on the device (one tensor) as the list of the plan's scales, highest
+        resolution first, from one target-kernel launch; anything else as it is."""
+        if getattr(self, "enable_deep_supervision", False) and not isinstance(target, list):
+            return DS.downsample_targets(target, self._ds_scales())
+        return target
+
+    def set_deep_supervision_enabled(self, enabled: bool):
+        """Switches the network's deep-supervision outputs, as the reference trainer does around its final validation
+        (nnUNetTrainer.py:1147, :1292); a trainer without deep supervision keeps them off whatever `enabled` says."""
+        mod = self.network.module if getattr(self, "is_ddp", False) else self.network
+        mod = getattr(mod, "_orig_mod", mod)
+        mod.decoder.deep_supervision = bool(enabled and getattr(self, "enable_deep_supervision", False))
 
     # ---- training step on the native path (nnUNetTrainer.py:486-489, 899-929)
     def configure_optimizers(self):
@@ -195,24 +231,23 @@ class DinoUNetTrainer(_Base):
     def train_step(self, batch: dict) -> dict:
         from .train_path import train_step
         data = batch["data"].to(self.device, non_blocking=True)
-        target = batch["target"]
-        if isinstance(target, list):
-            target = target[0]
-        target = target.to(self.device, non_blocking=True)
+        ds = getattr(self, "enable_deep_supervision", False)
+        target = self._target_to_device(batch["target"], ds and not DinoUNetTrainer._device_augmentation)
         if DinoUNetTrainer._device_augmentation:
             data, target = self._device_augmenter()(data, target)
+        # the device pipeline's target is downsampled after it (the host pipeline made no scales, PassThroughTransforms)
+        target = self._ds_targets(target)
         net = self.network.module if hasattr(self.network, "module") else self.network
         loss = train_step(net, self.loss, self.optimizer, data, target)
         return {"loss": loss.cpu().numpy()}
 
     def validation_step(self, batch: dict) -> dict:
         """One online-validation batch: native forward, then loss + hard tp/fp/fn in one fused pass over the logits
-        (argmax per class for label maps, sigmoid > 0.5 per region with the ignore channel as a weight for regions)."""
+        (argmax per class for label maps, sigmoid > 0.5 per region with the ignore channel as a weight for regions).
+        With deep supervision: the loss over every scale, the counts from the full-resolution output and target."""
         data = batch["data"].to(self.device, non_blocking=True)
-        target = batch["target"]
-        if isinstance(target, list):
-            target = target[0]
-        target = target.to(self.device, non_blocking=True)
+        target = self._target_to_device(batch["target"], getattr(self, "enable_deep_supervision", False))
+        target = self._ds_targets(target)
         with torch.no_grad():
             output = self.network(data)
         del data
@@ -247,6 +282,7 @@ class DinoUNetTrainer(_Base):
         if self.configuration_manager.next_stage_names is not None:
             raise NotImplementedError("the final validation on the device does not predict for next stages "
                                       f"({self.configuration_manager.next_stage_names})")
+        self.set_deep_supervision_enabled(False)
         self.network.eval()
         net = self.network.module if self.is_ddp else self.network
         net.repack()   # the optimizer changed the weights in place since the engine packed them
@@ -298,6 +334,7 @@ class DinoUNetTrainer(_Base):
             self.print_to_log_file("Validation complete", also_print_to_console=True)
             self.print_to_log_file("Mean Validation Dice: ", (metrics["foreground_mean"]["Dice"]),
                                    also_print_to_console=True)
+        self.set_deep_supervision_enabled(True)
 
 
 #: threads that export and write the final validation's cases; their host work overlaps the next prediction

@@ -402,6 +402,22 @@ int b2u_aug_noise_field(uint64_t seed, int32_t B, int32_t C, int64_t n, double* 
 int b2u_dl_crop(const void* staged, const int64_t* desc, int32_t B, int32_t C, int32_t H, int32_t W, int32_t mode,
                 const int32_t* regions, int32_t R, float* data, void* target, b2u_stream_t stream);
 
+/* ---- Deep-supervision targets (nnUNetTrainer.py:770-772, :799-801 DownsampleSegForDSTransform2(scales, order=0)):
+ * src [B, C, H, W] (dtype B2U_DS_INT16 label maps or B2U_DS_FP32 label maps / region channels); for each of nscales
+ * scales with integer factors (fy, fx) dividing (H, W), dst[s] [B, C, H/fy, W/fx] of src's dtype holds
+ * src[.., fy*oy + fy/2, fx*ox + fx/2] (skimage resize order 0, mode "edge": the nearest input sample, ties rounded up).
+ * Other factors are rejected before the launch.  One launch for every scale. */
+#define B2U_DS_MAX_SCALES 4
+#define B2U_DS_INT16 0
+#define B2U_DS_FP32 1
+typedef struct b2u_ds_targets_params {
+  const void* src;
+  int32_t dtype, B, C, H, W, nscales;
+  int32_t fy[B2U_DS_MAX_SCALES], fx[B2U_DS_MAX_SCALES];
+  void* dst[B2U_DS_MAX_SCALES];
+} b2u_ds_targets_params;
+int b2u_ds_targets(const b2u_ds_targets_params* p, b2u_stream_t stream);
+
 /* ---- Dice + cross-entropy loss and online-validation statistics on the logits of the forward path
  * (training/loss/compound_losses.py:31-56 `DC_and_CE_loss`, dice.py:72-119 `MemoryEfficientSoftDiceLoss`,
  * robust_ce_loss.py:12-16, built at nnUNetTrainer.py:363-365; consumer nnUNetTrainer.py:961-1005 `validation_step`).
@@ -489,7 +505,9 @@ int b2u_se_apply(const void* t, const void* sc, int64_t ldsc, const float* gate,
                  int32_t C, int32_t dtype, b2u_stream_t stream);
 
 /* Final InstanceNorm + LeakyReLU + 1x1 segmentation head + argmax (dinounet_training.py:597,619; nnUNetTrainer.py:977):
- *   x 16-bit [B*rows, C]; logits NCHW fp32 [B, ncls, rows]; labels uint8 [B, rows] (may be NULL). */
+ *   x 16-bit [B*rows, C]; logits NCHW fp32 [B, ncls, rows]; labels uint8 [B, rows] (may be NULL).  C = 32 (the last
+ *   decoder stage), or 64 / 128 (the deep-supervision heads seg_layers[1] / [0] on the earlier stages) with
+ *   ncls * C <= 128 * 32. */
 int b2u_seg_head(const void* x, const float* sums, const float* gamma, const float* beta, float eps, const float* w,
                  const float* b, float* logits, uint8_t* labels, int32_t B, int32_t rows, int32_t C, int32_t ncls,
                  int32_t dtype, b2u_stream_t stream);
